@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the hot path on B200 (one JSON line on stdout, rank 0).
+"""bench.py — throughput of the hot path on H100 (one JSON line on stdout, rank 0).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -18,9 +18,13 @@ barrier and the max-over-ranks time.
              inputs -> H2D -> forward -> D2H of the (B,3,T,96,96) result, every step.
   roofline   tensor-core bound: algorithmic FLOPs (7.934 GFLOP/crop, SURVEY.md §8d) of the conv kernel
              launches of one step / their summed per-launch CUDA-event durations (measured live, after the
-             timed region), against MEASURED_PEAKS.json's sustained bf16 figure (fp16 runs at the same rate).
+             timed region), against the H100 SXM data sheet's dense fp16 rate (989 TFLOP/s at 700 W).
   cpu_baseline  the oracle port (oracle/w2l_oracle.py, torch CPU fp32 = the reference's own arithmetic) on
              the host cores, N=128 4-D batch (inference.py's default batch), rank 0 at N=1 only.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller as float32 .npy
+files (inference: a seeded sample of whole windows of the (B,3,T,96,96) result, at most 64 MB; training: the step's
+losses), so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -38,13 +42,26 @@ METRIC = "96x96 face-crops/sec (B=128, T=5, mel 80x16)"
 B_DEFAULT, T_DEFAULT = 128, 5
 
 
-def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return {"tflops": float(d["bf16_tflops_sustained"]), "tflops_burst": float(d["bf16_tflops"]),
-                "hbm_gbs": float(d["hbm_gbs"]), "src": "measured"}
-    return {"tflops": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "src": "fallback"}
+# NVIDIA H100 SXM data sheet (700 W): dense fp16 / bf16 tensor rate and HBM3 bandwidth.  A card with a lower power limit
+# or clocks reaches less; the JSON line reports the card's clocks beside the result.
+H100_PEAKS = {"tflops": 989.0, "hbm_gbs": 3350.0, "src": "H100 SXM data sheet, dense fp16, 700 W"}
+DUMP_BYTES_MAX = 64 * 10**6
+
+
+def dump_outputs(out_dir, arrays):
+    """name -> array (torch or numpy) as out_dir/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().float().cpu().numpy() if hasattr(a, "detach") else np.asarray(a, dtype=np.float32)
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+
+
+def window_sample(B, per_window_bytes):
+    """Seeded choice of whole windows whose float32 outputs fit DUMP_BYTES_MAX (all of them when they fit)."""
+    import numpy as np
+    k = max(1, min(B, DUMP_BYTES_MAX // per_window_bytes))
+    return np.sort(np.random.default_rng(0).choice(B, size=k, replace=False))
 
 
 class ClockSampler:
@@ -96,8 +113,8 @@ class ClockSampler:
 
 
 def pick_threads(sd, O, torch):
-    """torch's CPU conv does not scale to every hardware thread of a large host (128 threads were 8x SLOWER than
-    32 on the B200 box): calibrate on a small batch and give the reference arm its best thread count."""
+    """torch's CPU conv does not scale to every hardware thread of a large host: calibrate on a small batch and give
+    the reference arm its best thread count."""
     cores = os.cpu_count() or 1
     cands = sorted({c for c in (8, 16, 32, 64, cores) if c <= cores})
     mel, face = O.make_generator_inputs(8, 1)
@@ -264,7 +281,7 @@ def measure_extra(dev):
     return out
 
 
-def measure_train(dev, rank, world, steps, warmup, B=64, T=5, syncnet_wt=0.03, profile_out=None):
+def measure_train(dev, rank, world, steps, warmup, B=64, T=5, syncnet_wt=0.03, profile_out=None, dump_dir=None):
     """BASELINE configs[4]: one wav2lip_train.py:210-231 iteration per step (generator train-mode forward, get_sync_loss
     through the frozen expert, L1, backward, gradient all-reduce over NCCL when world > 1, Adam), bf16 operands, B=64
     windows x T=5 frames per GPU, everything native (w2l_wav2lip_train_step).  Inputs resident on the device; CUDA-event
@@ -314,6 +331,8 @@ def measure_train(dev, rank, world, steps, warmup, B=64, T=5, syncnet_wt=0.03, p
     syn_f = ctx.lib.w2l_train_flops(ctx.h, _lib.NET_SYNCNET)
     flop = 3.0 * gen_f + 2.0 * syn_f       # forward + dgrad + wgrad of the generator; forward + dgrad of the frozen expert
     lv = [float(v) for v in losses.cpu()]
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, {"losses": losses})   # (sync, l1, ..., total) of the last timed step
     n_param = sum(p.numel() for p in model.parameters())
     if profile_out and rank == 0:
         rows = ctx.train_profile(_lib.NET_GENERATOR, iters=3, stream=stream.cuda_stream) + \
@@ -346,12 +365,14 @@ def run_reference(args, rank, world):
     with torch.no_grad():
         for _ in range(max(1, min(args.warmup, 1))):
             O.generator_forward(sd, mel, face)
-        steps = max(1, min(args.steps, 3))   # ~14 s per step on the box's host: the whole arm stays under ~2 minutes
+        steps = args.steps
         t0 = time.perf_counter()
         for _ in range(steps):
-            O.generator_forward(sd, mel, face)
+            out = O.generator_forward(sd, mel, face)
         dt = (time.perf_counter() - t0) / steps
     v = n / dt
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"generator_out": out[window_sample(B, out[0].numel() * 4)]})
     line = {
         "impl": "reference", "metric": METRIC, "value": v, "unit": "crops/s", "n_gpus": args.gpus, "steps": steps,
         "warmup": args.warmup, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -379,6 +400,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the SyncNet / disc / mel side measurements")
     ap.add_argument("--profile-out", default=None, help="write the per-launch table to this file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one returned as DIR/<name>.npy (float32)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="weak (default, the driver's mode): --batch windows PER GPU.  strong: --batch is the GLOBAL batch, split over the ranks")
     ap.add_argument("--workload", default="infer", choices=["infer", "train"],
@@ -401,7 +424,7 @@ def main():
     if args.warmup < 3:
         args.warmup = 3
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200; there is no CPU path (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100; there is no CPU path (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -413,7 +436,8 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     if args.workload == "train":
         tb = 64 if args.batch == B_DEFAULT else args.batch
-        r = measure_train(dev, rank, world, args.steps, args.warmup, B=tb, T=args.frames, profile_out=args.profile_out)
+        r = measure_train(dev, rank, world, args.steps, args.warmup, B=tb, T=args.frames, profile_out=args.profile_out,
+                          dump_dir=args.dump_outputs)
         if rank == 0:
             line = {"metric": "wav2lip_train.py iterations: 96x96 face-crops/sec trained (B=64/GPU, T=5, bf16)", "value": r["crops_per_s"],
                     "unit": "crops/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": r["ms_per_step"],
@@ -487,6 +511,8 @@ def main():
             per_rank_ms = [float(v) for v in box]
         ms = max_over_ranks(ms, dev)
         clocks = sampler.stop(t_wall0, t_wall1) if rank == 0 else None
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"generator_out": out[torch.from_numpy(window_sample(B, out[0].numel() * 4)).to(dev)]})
         ms_per_step = ms / args.steps
         value = world * N * args.steps / (ms * 1e-3)
 
@@ -545,27 +571,17 @@ def main():
         # ---- roofline: per-launch CUDA-event timing of the conv kernel family (after the timed region) ----
         out = model(mel_d, face_d)  # make the full-batch plan the profiled one again (the host path runs chunk plans)
         torch.cuda.synchronize(dev)
-        peaks = load_peaks()
+        peaks = H100_PEAKS
         prof = ctx.profile_plan(_lib.NET_GENERATOR, iters=3, stream=stream.cuda_stream)
         conv_ms = sum(m for _, m, _ in prof)
         conv_flop = sum(f for _, _, f in prof)
         achieved = conv_flop / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-        roofline = {"bound": "tensor", "kernel": "conv_igemm_kernel<BN,BK> (tcgen05 implicit GEMM, all conv launches of one step)",
+        roofline = {"bound": "tensor", "kernel": "conv_igemm_kernel / conv_patch_kernel / convt_fused_kernel (wgmma implicit GEMM, all conv launches of one step)",
                     "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
-                    "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['src']}); fp16 operands run at the bf16 rate",
+                    "peak_source": peaks["src"],
                     "launches_per_step": len(prof), "conv_ms_per_step_isolated": conv_ms,
                     "share_of_step": conv_ms / ms_per_step if ms_per_step > 0 else None,
-                    "whole_step_tflops": value / world * FLOP_PER_CROP / 1e12,
-                    "traffic": None}
-        # DRAM bytes of the same launches from the committed ncu capture (profiles/), valid for the default workload
-        tname = next((n for n in ("r2_final_ncu_dram_per_step.json", "r1_final_ncu_dram_per_step.json")
-                      if os.path.exists(os.path.join(ROOT, "profiles", n))), None)
-        if tname and (B, T) == (B_DEFAULT, T_DEFAULT):
-            tj = json.load(open(os.path.join(ROOT, "profiles", tname)))
-            roofline["traffic"] = tj["dram_read_bytes"] + tj["dram_write_bytes"]
-            roofline["traffic_note"] = ("dram__bytes_read+write summed over the %d conv launches of one step (ncu, profiles/"
-                                        "%s); algorithmic conv in+out bytes per step = %.2f GB"
-                                        % (tj["launches"], tname, (4.81e6 + 4.49e6) * 2 * N / 1e9))
+                    "whole_step_tflops": value / world * FLOP_PER_CROP / 1e12}
         if args.profile_out and rank == 0:
             with open(args.profile_out, "w") as f:
                 f.write(f"# per-launch CUDA-event times, B={B} T={T} (N={N}), {len(prof)} conv launches, sum {conv_ms:.3f} ms\n")
@@ -597,7 +613,7 @@ def main():
             "config": {"workload": f"BASELINE configs[1] at the metric's B={B}, T={T}: Wav2Lip.forward eval, {N} crops/GPU/step, fp32 NCHW in/out",
                        "per_gpu_batch": N, "global_batch": N * world, "parallelism": f"replicas x{world}, batch-sharded, no collective",
                        "weights": "seeded random (reference default-init statistics + randomised BatchNorm)",
-                       "l2": "inputs larger than L2 (141 MB face + activations >> 126 MB), no explicit flush",
+                       "l2": "inputs larger than L2 (141 MB face + activations >> 50 MB), no explicit flush",
                        "precision": "fp16 operands / fp32 accumulate+epilogue (TF32-class mantissa)"},
             "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "cpu_baseline": cpu,
             "extra": extra,

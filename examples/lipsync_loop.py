@@ -1,4 +1,4 @@
-"""The hot loop of the reference's inference.py (:224-271) on the B200 core, with synthetic crops and audio:
+"""The hot loop of the reference's inference.py (:224-271) on the H100 core, with synthetic crops and audio:
 
     wav --audio.melspectrogram--> mel (80,F) --audio.mel_chunks(fps)--> (n_frames,1,80,16)       inference.py:225, 231-240
     uint8 96x96 BGR crops (what cv2.resize at :126 produces)  +  mel chunks

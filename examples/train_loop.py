@@ -1,4 +1,4 @@
-"""The training loops of the reference on the B200 core, with synthetic batches (there is no dataset here):
+"""The training loops of the reference on the H100 core, with synthetic batches (there is no dataset here):
 
   --mode script   the statements of wav2lip_train.py:210-231 as the script writes them — `model.train()`, `g = model(indiv_mels, x)`,
                   `get_sync_loss` through the frozen expert (left in train mode, :187-189), `recon_loss`, `loss.backward()`,

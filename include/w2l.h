@@ -1,5 +1,5 @@
 /*
- * w2l.h — C-ABI of the B200-native Wav2Lip compute core (libw2l.so).
+ * w2l.h — C-ABI of the H100-native Wav2Lip compute core (libw2l.so).
  *
  * The reference (Rudrabha/Wav2Lip) has no FFI: its boundary is the Python module surface
  * `models` / `audio` that the scripts import by bare name.  Each entry point below replaces
@@ -17,7 +17,7 @@
  *    asynchronous on that stream unless stated otherwise.
  *  - a context is bound to one device and is not thread safe (one context per GPU / stream).
  *  - there is NO CPU fallback: every compute entry point fails with W2L_ENODEV when no
- *    sm_100 device is usable.
+ *    sm_90 (H100) device is usable.
  */
 #ifndef W2L_H_
 #define W2L_H_
@@ -33,7 +33,7 @@ extern "C" {
 /* error codes */
 #define W2L_OK        0
 #define W2L_EINVAL   -1   /* bad argument / shape */
-#define W2L_ENODEV   -2   /* no usable sm_100 CUDA device */
+#define W2L_ENODEV   -2   /* no usable sm_90 CUDA device */
 #define W2L_ECUDA    -3   /* CUDA runtime / driver error (see w2l_last_error) */
 #define W2L_ENOMEM   -4
 #define W2L_ESTATE   -5   /* e.g. forward before weights were loaded */
@@ -220,8 +220,8 @@ int w2l_mel_basis_host(float* out_host);
 
 /* ---- training step (scope row f1): wav2lip_train.py:210-231, color_syncnet_train.py:146-163, hq_wav2lip_train.py:213-255 ----
  * Train-mode forward (BatchNorm on batch statistics over the T*B flatten, conv.py:8-11 / wav2lip.py:93-94; running
- * averages updated with momentum 0.1) and backward through every block, as kernels: conv / dgrad on the tcgen05 conv
- * kernels, wgrad on a tcgen05 kernel whose K dimension is the pixel index, BatchNorm / ReLU / residual passes,
+ * averages updated with momentum 0.1) and backward through every block, as kernels: conv / dgrad on the wgmma conv
+ * kernels, wgrad on a wgmma kernel whose K dimension is the pixel index, BatchNorm / ReLU / residual passes,
  * loss gradients, multi-tensor Adam, bucketed NCCL all-reduce of the gradients.  bf16 operands, fp32 accumulation,
  * fp32 master parameters and gradients (the context must be created with W2L_PREC_BF16).
  *

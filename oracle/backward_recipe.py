@@ -53,7 +53,7 @@ def conv_dgrad(dz: torch.Tensor, w: torch.Tensor, row: Row, in_hw: Tuple[int, in
 
 
 def conv_wgrad(x: torch.Tensor, dz: torch.Tensor, row: Row) -> torch.Tensor:
-    """Per-tap GEMMs with the pixel index as the contraction dimension (what the tcgen05 wgrad kernel will do)."""
+    """Per-tap GEMMs with the pixel index as the contraction dimension (what the wgrad kernel does)."""
     kind, cin, cout, k, s, p, op, _res = row
     (kh, kw), (sh, sw), (ph, pw) = _pair(k), _pair(s), _pair(p)
     x, dz = Q(x), Q(dz)

@@ -57,8 +57,8 @@ CASES = [
     ("ragged 5x7", "c", 64, 64, 3, 1, 1, 0, True, 3, 5, 7),
     ("ragged 13x11 s2", "c", 32, 64, 3, 2, 1, 0, False, 5, 13, 11),
     ("N=131 3x3 spatial", "c", 64, 64, 3, 1, 1, 0, True, 131, 3, 3),
-    # batches large enough (>= 2 x 148 units of 256 pixels) for conv_swap_kernel, the channel-major variant of the 128-channel
-    # tiles (csrc/conv_swap.cuh): residual, three channel tiles, ragged boxes, strided, transposed-conv phases
+    # batches large enough for many 128-row tiles per SM at 128-channel tiles (the ids keep the names of a retired variant):
+    # residual, three channel tiles, ragged boxes, strided, transposed-conv phases
     ("swap 3x3 128 res 24x24 N=140", "c", 128, 128, 3, 1, 1, 0, True, 140, 24, 24),
     ("swap 3x3 384 res 12x12 N=190", "c", 384, 384, 3, 1, 1, 0, True, 190, 12, 12),
     ("swap ragged 23x24 128 res N=150", "c", 128, 128, 3, 1, 1, 0, True, 150, 23, 24),

@@ -1,5 +1,5 @@
 """Training row (SURVEY.md section 8 f1), operator level: one conv.py block in TRAIN mode — forward on batch statistics
-and the full backward (dx via the dgrad launches, dW via the tcgen05 wgrad kernel + split-K reduction, dgamma / dbeta /
+and the full backward (dx via the dgrad launches, dW via the wgmma wgrad kernel + split-K reduction, dgamma / dbeta /
 dbias, running-average update) — through the C-ABI entry `w2l_conv_block_train`, for every distinct block geometry of
 the three networks, against oracle/backward_recipe.py (float64; itself equal to torch autograd, tests/
 test_backward_recipe.py).

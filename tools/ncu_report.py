@@ -1,4 +1,4 @@
-"""Turns ncu CSV logs into the summaries committed under profiles/.  Test/measurement infrastructure.
+"""Turns ncu CSV logs into per-launch summaries.  Test/measurement infrastructure.
 
   launches  <ncu --metrics gpu__time_duration.sum --csv log>            -> per-kernel time shares of the whole command
   step      <ncu --metrics dram__bytes_read.sum,... --csv log> <names>  -> per-step DRAM bytes / tensor-pipe % (JSON + table)

@@ -11,7 +11,7 @@ with torch.no_grad():
     g = Wav2Lip().cuda().eval()
     y = g(torch.rand(3, 1, 80, 16).cuda(), torch.rand(3, 6, 96, 96).cuda())
     y5 = g(torch.rand(2, 2, 1, 80, 16).cuda(), torch.rand(2, 6, 2, 96, 96).cuda())
-    y6 = g(torch.rand(6, 1, 80, 16).cuda(), torch.rand(6, 6, 96, 96).cuda())   # enough tiles for the row-stack kernels
+    y6 = g(torch.rand(6, 1, 80, 16).cuda(), torch.rand(6, 6, 96, 96).cuda())   # enough tiles for the patch kernels
     ys = list(g.infer_stream(iter([(torch.rand(5, 1, 80, 16), torch.rand(5, 6, 96, 96)),
                                    (torch.rand(2, 1, 80, 16), torch.randint(0, 256, (2, 96, 96, 3), dtype=torch.uint8))])))
     u = g.infer_u8(torch.rand(3, 1, 80, 16).cuda(), torch.randint(0, 256, (3, 96, 96, 3), dtype=torch.uint8).cuda())
@@ -28,7 +28,7 @@ with torch.no_grad():
     cr = g.crop_resize(frames, boxes)
     pa = g.paste(u[:2], frames, boxes)
     fr = g.infer_frames(torch.rand(2, 1, 80, 16).cuda(), frames, boxes)
-    # conv_swap_kernel (needs >= 296 units of 256 pixels): a 128-channel residual block and a transposed-conv phase set
+    # many units of 128-channel tiles: a 128-channel residual block and a transposed-conv phase set
     from wav2lip_b200.models.conv import Conv2d, Conv2dTranspose
     sw = Conv2d(128, 128, 3, 1, 1, residual=True).cuda().eval()(torch.rand(140, 128, 24, 24).cuda())
     swt = Conv2dTranspose(320, 128, 3, 2, 1, 1).cuda().eval()(torch.rand(150, 320, 12, 12).cuda())

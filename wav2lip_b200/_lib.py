@@ -1,7 +1,7 @@
 """ctypes binding of libw2l.so — the declarations of include/w2l.h, nothing else.
 
 The library is built in-tree by `python -c "import __graft_entry__ as g; g.build()"`
-(nvcc -gencode arch=compute_100a,code=sm_100a).  If it is missing, importing this module still
+(nvcc -gencode arch=compute_90a,code=sm_90a).  If it is missing, importing this module still
 works (so that error messages are useful) but any use raises W2LError: there is no fallback path.
 """
 from __future__ import annotations

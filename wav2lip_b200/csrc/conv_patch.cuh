@@ -1,6 +1,6 @@
 // conv_patch.cuh — "patch" variant of the implicit-GEMM conv for layers with few channels, where the generic
-// kernel (conv_tcgen05.cuh) is bound by L2->SM operand traffic because it re-loads the input box for every
-// filter tap (profiles/r1_v1_ncu_full_conv_summary.txt).  Used for
+// kernel (conv_igemm.cuh) is bound by L2->SM operand traffic because it re-loads the input box for every
+// filter tap.  Used for
 //   * 3x3 / stride 1 / pad 1 blocks with Cout <= 64 (conv.py:5-19 at wav2lip.py:16-22,40-45,79-83; the
 //     80->32 output block with the fused 1x1+sigmoid head, wav2lip.py:83-85),
 //   * the output phases of the last transposed conv (conv.py:33-44 at wav2lip.py:79), and
@@ -13,29 +13,29 @@
 //     chunk (PW x PH pixels x BK channels, e.g. 10 x 18 for a 3x3 conv; out-of-bounds zero-filled by TMA =
 //     the conv padding).
 // Every tap is a shifted VIEW of that patch: in the K-major swizzled layout a pixel is one shared-memory row,
-// the 8 pixels of an output row are 8 consecutive rows (one UMMA 8-row group) and the next output row starts
-// exactly one patch row (PW pixels) further, so the UMMA descriptor of tap t is
+// the 8 pixels of an output row are 8 consecutive rows (one 8-row group of the wgmma descriptor) and the next output
+// row starts exactly one patch row (PW pixels) further, so the descriptor of tap t is
 //     start = patch + tap_row[t] * row_bytes,     stride-byte-offset = PW * row_bytes.
-// The hardware swizzle is a function of the shared-memory ADDRESS bits (TMA writes and UMMA reads apply the
-// same XOR), so group starts need not be aligned to the 8-row swizzle atom — verified on B200 by the parity
-// tests.  Operand traffic per tile drops from taps x (A + B) to one patch.
+// The hardware swizzle is a function of the shared-memory ADDRESS bits (TMA writes and wgmma reads apply the
+// same XOR), so group starts need not be aligned to the 8-row swizzle atom.  Operand traffic per tile drops from
+// taps x (A + B) to one patch.
 //
-// With K this short the epilogue, not the main loop, is the critical path (the first version, with one global
-// 16-byte access per thread and row, was L1TEX-bound at 88 %: profiles/r1_v2_ncu_patch_summary.txt), so
-//   * there are TWO epilogue warp groups (one per TMEM accumulator stage, alternating tiles);
+// Two consumer warpgroups take alternate tiles; each issues the wgmma chain of its tile into registers and runs
+// the epilogue, so one group's epilogue overlaps the other's MMAs.  The ring has an even number of stages, so a
+// stage is always consumed by the same warpgroup and its parity waits are in order.  In the epilogue
 //   * the residual of a residual block is the block's own input, i.e. the centre of the patch that is already
-//     in shared memory: it is read from there (the epilogue, not the MMA commit, then releases the patch);
+//     in shared memory: it is read from there (the warpgroup releases the patch after that read);
 //   * results are staged in swizzled shared memory and written with ONE TMA tensor store per tile (which also
 //     clips ragged edges), instead of 128 threads x 8 scattered 16-byte stores;
 //   * scale/shift/head weights come from the constant bank (kernel params).
 #pragma once
 
-#include "conv_tcgen05.cuh"
+#include "conv_igemm.cuh"
 
 namespace w2l {
 
 constexpr int kPatchTileW = 8, kPatchTileH = 16;  // output tile (pixels)
-constexpr int kPatchThreads = 384;       // warps: 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-7 epilogue A, 8-11 epilogue B
+constexpr int kPatchThreads = 384;       // warps: 0 TMA, 1 barrier init, 2-3 idle, 4-7 consumer A, 8-11 consumer B
 constexpr int kPatchMaxTaps = 9;
 constexpr int kPatchMaxStages = 8;
 
@@ -47,14 +47,13 @@ struct alignas(64) PatchParams {
     int has_out2;
     int tiles_x, tiles_y;   // tiles per image
     int kc;                 // channel chunks of BK
-    int stages;             // depth of the patch ring
+    int stages;             // depth of the patch ring (even)
     int PW, PH;             // patch size in pixels
     int ox, oy;             // patch origin relative to the tile origin (-1,-1 for a padded 3x3)
     int ntaps;
     int patch_bytes;        // PW*PH*BK*2 (TMA transaction size)
     int patch_stride;       // ring slot size (patch_bytes rounded up to 1024)
     int tap_row[kPatchMaxTaps];  // first patch row (pixel index) of each tap's view
-    int pair;               // 1: process two tiles at a time on two accumulators (needs a ring of >= 4 patches)
     int res_row;            // >= 0: the residual IS the block input: patch row of the tile's first pixel (centre tap)
     EpiParams ep;
     float cscale[64], cshift[64];  // folded BatchNorm, constant bank
@@ -66,12 +65,13 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     pdl_launch_dependents();
     constexpr int kSlab = BN * BK * 2;  // one (tap, chunk) weight slab
     constexpr int kRowBytes = BK * 2;
-    constexpr int kTmemCols = (4 * BN <= 32) ? 32 : (4 * BN <= 64) ? 64 : (4 * BN <= 128) ? 128 : 256;  // 2 tiles in flight x 2 stages
+    constexpr int CW = BN < 32 ? BN : 32;
     static_assert(BN <= 64, "resident-weight variant is for narrow layers");
     static_assert(!kHead || BN == 32, "fused head expects the 32-channel output block");
 
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t smem_raw_u32 = smem_u32(smem_raw);
+    const uint32_t smem_base = (smem_raw_u32 + 1023u) & ~1023u;
     const int kc = p.kc;
     const int stages = p.stages;
     const int ntaps = p.ntaps;
@@ -79,13 +79,11 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     const uint32_t a_base = w_base + static_cast<uint32_t>(ntaps * kc) * kSlab;
     const uint32_t stg_base = a_base + static_cast<uint32_t>(stages * kc) * p.patch_stride;  // a stage = all chunks of one tile
     constexpr uint32_t kStgBytes = ((kTileM * BN * 2 + 1023) / 1024) * 1024;                  // one staging tile per group
-    const uint32_t bar_base = stg_base + 2u * kStgBytes;
+    const uint32_t xb_base = stg_base + 2u * kStgBytes;
+    const uint32_t bar_base = xb_base + 2u * xbuf_bytes<32>();
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kPatchMaxStages + s); };
-    auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * kPatchMaxStages + a); };       // 4 accumulator slots
-    auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * kPatchMaxStages + 4 + a); };
-    const uint32_t w_bar = bar_base + 8u * (2 * kPatchMaxStages + 8);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * kPatchMaxStages + 9);
+    const uint32_t w_bar = bar_base + 8u * (2 * kPatchMaxStages);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -99,22 +97,13 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < stages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), p.res_row >= 0 ? 5 : 1);  // MMA commit (+ the 4 epilogue warps that read the residual)
-        }
-        for (int a = 0; a < 4; ++a) {
-            mbar_init(tfull_bar(a), 1);
-            mbar_init(tempty_bar(a), 4);
+            mbar_init(empty_bar(s), 4);  // the 4 warps of the warpgroup that consumed the patch (MMAs retired, residual read)
         }
         mbar_init(w_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc<kTmemCols>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
     pdl_wait();  // everything above overlaps the previous kernel's tail; global memory is touched only below
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
     const int tiles_per_img = p.tiles_x * p.tiles_y;
     const int total_tiles = tiles_per_img * p.ep.N;
@@ -140,74 +129,10 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
                 if (++stage == stages) { stage = 0; phase ^= 1u; }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // =============================== MMA issuer ===============================
-        constexpr uint32_t idesc = make_idesc<BN, kBF16>();
-        // descriptor halves: hi = [SBO | version | layout], lo = [start address >> 4 | LBO = 1]
-        constexpr uint32_t kLayout = (BK == 64) ? 2u : (BK == 32) ? 4u : 6u;
-        const uint32_t a_hi = ((static_cast<uint32_t>(p.PW) * kRowBytes) >> 4) | (1u << 14) | (kLayout << 29);
-        constexpr uint32_t b_hi = ((8u * kRowBytes) >> 4) | (1u << 14) | (kLayout << 29);
-        uint32_t tap_off[kPatchMaxTaps];
-#pragma unroll
-        for (int t = 0; t < kPatchMaxTaps; ++t) tap_off[t] = (t < ntaps ? p.tap_row[t] : 0) * kRowBytes;
-        mbar_wait(w_bar, 0);
-        // Dependent MMAs on ONE accumulator issue only every ~90 cycles whatever N is (measured: 85-110 cycles per
-        // M=128,K=16 instruction for N = 16..64), so two tiles are processed together and their MMAs alternate
-        // between two independent TMEM accumulators; with the two draining ones that makes 4 accumulator slots.
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int u = 0;; ++u) {
-            const int tile0 = blockIdx.x + (p.pair ? 2 * u : u) * gridDim.x;
-            if (tile0 >= total_tiles) break;
-            const bool two = p.pair && (tile0 + static_cast<int>(gridDim.x) < total_tiles);
-            const int slot = (u & 1) * 2;
-            const uint32_t acc_phase = (u >> 1) & 1u;
-            const int stage_a = stage;
-            const uint32_t phase_a = phase;
-            if (++stage == stages) { stage = 0; phase ^= 1u; }
-            const int stage_b = stage;
-            const uint32_t phase_b = phase;
-            if (two) { if (++stage == stages) { stage = 0; phase ^= 1u; } }
-            mbar_wait(tempty_bar(slot), acc_phase ^ 1u);
-            if (two) mbar_wait(tempty_bar(slot + 1), acc_phase ^ 1u);
-            mbar_wait(full_bar(stage_a), phase_a);
-            if (two) mbar_wait(full_bar(stage_b), phase_b);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t tmem_a = tmem_base + slot * BN;
-                const uint32_t tmem_b = tmem_a + BN;
-                for (int c = 0; c < kc; ++c) {
-                    const uint32_t patch_a = a_base + (stage_a * kc + c) * p.patch_stride;
-                    const uint32_t patch_b = a_base + (stage_b * kc + c) * p.patch_stride;
-#pragma unroll
-                    for (int tap = 0; tap < kPatchMaxTaps; ++tap) {
-                        if (tap < ntaps) {
-                            const uint32_t a_lo = ((patch_a + tap_off[tap]) >> 4) | 0x10000u;
-                            const uint32_t a2_lo = ((patch_b + tap_off[tap]) >> 4) | 0x10000u;
-                            const uint32_t b_lo = ((w_base + (tap * kc + c) * kSlab) >> 4) | 0x10000u;
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
-                                const uint64_t bdesc = (static_cast<uint64_t>(b_hi) << 32) | (b_lo + 2u * k);
-                                const uint32_t accum = (c | tap | k) != 0 ? 1u : 0u;
-                                tc_mma_f16(tmem_a, (static_cast<uint64_t>(a_hi) << 32) | (a_lo + 2u * k), bdesc, idesc, accum);
-                                if (two)
-                                    tc_mma_f16(tmem_b, (static_cast<uint64_t>(a_hi) << 32) | (a2_lo + 2u * k), bdesc, idesc, accum);
-                            }
-                        }
-                    }
-                }
-                tc_commit(empty_bar(stage_a));
-                if (two) tc_commit(empty_bar(stage_b));
-                tc_commit(tfull_bar(slot));
-                if (two) tc_commit(tfull_bar(slot + 1));
-            }
-            __syncwarp();
-        }
     } else if (warp >= 4) {
-        // =============================== epilogue (two groups, one per accumulator stage) ===============================
-        const int grp = (warp - 4) >> 2;   // 0: tiles 0,2,4..  1: tiles 1,3,5..
-        const int q = (warp - 4) & 3;      // TMEM lane quarter = warp id % 4
+        // ============ consumer warpgroups (MMA + epilogue), alternating tiles: group g takes tiles g, g+2, .. ============
+        const int grp = (warp - 4) >> 2;
+        const int q = (warp - 4) & 3;
         const int row = q * 32 + lane;
         const int py = row >> 3, px = row & 7;  // GEMM row -> pixel inside the 8 x 16 tile
         const EpiParams& e = p.ep;
@@ -215,34 +140,44 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
         constexpr uint32_t kOutSwz = (kOutRow == 128) ? 7u : (kOutRow == 64) ? 3u : 1u;   // matches tmO's swizzle mode
         constexpr uint32_t kInSwz = (BK == 64) ? 7u : (BK == 32) ? 3u : 1u;
         const uint32_t stg = stg_base + grp * kStgBytes;
+        float* const xb = reinterpret_cast<float*>(smem_raw + (xb_base - smem_raw_u32) + grp * xbuf_bytes<32>());
         const bool leader = (q == 0 && lane == 0);
         const uint32_t bar_id = 1 + grp;  // named barrier of this group (0 is __syncthreads)
-        for (int u = 0;; ++u) {
-            // paired mode: group g takes the g-th tile of every pair; single mode: groups alternate tiles
-            if (!p.pair && (u & 1) != grp) continue;
-            const int it = p.pair ? 2 * u + grp : u;
+        // Every tap is a shifted view of the patch: the 8 pixels of an output row are 8 consecutive patch rows (one 8-row
+        // group of the descriptor) and the next output row starts one patch row (PW pixels) further.
+        const uint32_t sbo_a = static_cast<uint32_t>(p.PW) * kRowBytes;
+        uint32_t tap_off[kPatchMaxTaps];
+#pragma unroll
+        for (int t = 0; t < kPatchMaxTaps; ++t) tap_off[t] = (t < ntaps ? p.tap_row[t] : 0) * kRowBytes;
+        mbar_wait(w_bar, 0);
+        float acc[2][BN / 2];
+        for (int it = grp;; it += 2) {
             const int tile = blockIdx.x + it * gridDim.x;
             if (tile >= total_tiles) break;
-            const int uu = p.pair ? u : (u >> 1);      // how many times this group's accumulator slot has been used
-            const int acc = p.pair ? (u & 1) * 2 + grp : grp * 2;
-            const uint32_t acc_phase = p.pair ? ((u >> 1) & 1u) : (uu & 1u);
             const int stage = it % stages;
             const int n = tile / tiles_per_img;
             const int r = tile - n * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
             const int x = tx * kPatchTileW + px, y = ty * kPatchTileH + py;
 
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
+            mbar_wait(full_bar(stage), static_cast<uint32_t>(it / stages) & 1u);
+            wg_fence();
+            for (int c = 0; c < kc; ++c) {
+                const uint32_t patch = a_base + (stage * kc + c) * p.patch_stride;
+#pragma unroll
+                for (int tap = 0; tap < kPatchMaxTaps; ++tap)
+                    if (tap < ntaps)
+                        wg_mma_tile<BN, BK, kBF16>(acc, patch + tap_off[tap], sbo_a, w_base + (tap * kc + c) * kSlab, (c | tap) != 0);
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_fence_regs<BN / 2>(acc[0]);
+            wg_fence_regs<BN / 2>(acc[1]);
+            if (p.res_row < 0 && lane == 0) mbar_arrive(empty_bar(stage));  // the MMAs were the patch's last readers
+
             uint32_t v[BN];
 #pragma unroll
-            for (int c0 = 0; c0 < BN; c0 += 16) tmem_ld16(taddr + c0, v + c0);
-            tmem_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));  // accumulator drained: the MMA warp may reuse this TMEM stage
-
+            for (int c0 = 0; c0 < BN; c0 += CW) acc_to_rows<CW>(acc[0], acc[1], c0, xb, bar_id, v + c0);
             float f[BN];
 #pragma unroll
             for (int j = 0; j < BN; ++j) f[j] = fmaf(__uint_as_float(v[j]), p.cscale[j], p.cshift[j]);
@@ -318,10 +253,6 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
         }
         if (!kHead && leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 }  // namespace w2l

@@ -1,5 +1,5 @@
 // host_launch.cuh — kernel instantiation tables and the one function that launches a conv Op (generic / patch /
-// row-stack / fused transposed-conv kernel), with the per-device shared-memory attribute and the PDL launch attribute.
+// fused transposed-conv kernel), with the per-device shared-memory attribute and the PDL launch attribute.
 // Part of the single translation unit w2l_api.cu (included there, in this order).
 #pragma once
 
@@ -21,8 +21,7 @@ static ConvKernelEntry g_conv_kernels[] = {
     W2L_CONV_ENTRY(32, 16), W2L_CONV_ENTRY(32, 32), W2L_CONV_ENTRY(32, 64),
     W2L_CONV_ENTRY(64, 16), W2L_CONV_ENTRY(64, 32), W2L_CONV_ENTRY(64, 64),
     W2L_CONV_ENTRY(128, 16), W2L_CONV_ENTRY(128, 32), W2L_CONV_ENTRY(128, 64),
-    W2L_CONV_ENTRY(256, 64),
-    W2L_CONV_ENTRY_MT2(128, 64), W2L_CONV_ENTRY_MT2(64, 64), W2L_CONV_ENTRY_MT2(64, 32),
+    W2L_CONV_ENTRY_MT2(64, 64), W2L_CONV_ENTRY_MT2(64, 32),
     {32, 16, false, true, conv_igemm_kernel<32, 16, false, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, 256},
     {32, 16, true, true, conv_igemm_kernel<32, 16, true, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, 256},
 };
@@ -49,28 +48,6 @@ static PatchKernelEntry* find_patch_kernel(int BN, int BK, bool bf16, bool head)
     for (auto& e : g_patch_kernels)
         if (e.BN == BN && e.BK == BK && e.bf16 == bf16 && e.head == head) return &e;
     return nullptr;
-}
-
-typedef void (*RsKernelFn)(const RowStackParams);
-struct RsKernelEntry { int shape; bool bf16; RsKernelFn fn; uint64_t attr_set; };
-static RsKernelEntry g_rs_kernels[] = {
-    {0, false, conv_rowstack_kernel<32, 2, 3, 3, 16, false, true>, 0},
-    {0, true, conv_rowstack_kernel<32, 2, 3, 3, 16, true, true>, 0},
-    {1, false, conv_rowstack_kernel<16, 3, 7, 1, 0, false, false>, 0},
-    {1, true, conv_rowstack_kernel<16, 3, 7, 1, 0, true, false>, 0},
-    {2, false, conv_rowstack_kernel<32, 3, 7, 1, 0, false, false>, 0},
-    {2, true, conv_rowstack_kernel<32, 3, 7, 1, 0, true, false>, 0},
-};
-using RsCfg0 = RowStackCfg<32, 2, 3, 3, 16>;   // generator output block (+ head)
-using RsCfg1 = RowStackCfg<16, 3, 7, 1, 0>;    // generator first block (6 -> 16, 7x7 folded)
-using RsCfg2 = RowStackCfg<32, 3, 7, 1, 0>;    // disc first block (3 -> 32, 7x7 folded, LeakyReLU)
-struct RsShape { int PW, PH, tile_h, R, ndx, fixed, per_stage; };
-static RsShape rs_shape(int shape) {
-    switch (shape) {
-        case 0: return {RsCfg0::PW, RsCfg0::PH, RsCfg0::kTileH, 1, 3, RsCfg0::smem_bytes(0, true), RsCfg0::kStageStride};
-        case 1: return {RsCfg1::PW, RsCfg1::PH, RsCfg1::kTileH, 3, 1, RsCfg1::smem_bytes(0, false), RsCfg1::kStageStride};
-        default: return {RsCfg2::PW, RsCfg2::PH, RsCfg2::kTileH, 3, 1, RsCfg2::smem_bytes(0, false), RsCfg2::kStageStride};
-    }
 }
 
 typedef void (*CtKernelFn)(const ConvTParams);
@@ -120,28 +97,11 @@ static int launch_conv(w2l_ctx* ctx, const Op& op, cudaStream_t st, bool pdl = t
         ctx->launches++;
         return W2L_OK;
     }
-    if (op.rowstack) {
-        RsKernelEntry* e = nullptr;
-        for (auto& k : g_rs_kernels) if (k.shape == op.rs_shape && k.bf16 == ctx->bf16) e = &k;
-        if (!e) return fail(W2L_EINVAL, "no row-stack kernel for shape %d", op.rs_shape);
-        CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, kSmemBudget + kSmemExtra));
-        CK(launch_k(e->fn, op.grid, kRsThreads, op.dyn_smem, st, op.rs, pdl));
-        ctx->launches++;
-        return W2L_OK;
-    }
     if (op.patch) {
         PatchKernelEntry* e = find_patch_kernel(op.BN, op.BK, ctx->bf16, op.head);
         if (!e) return fail(W2L_EINVAL, "no patch kernel for BN=%d BK=%d head=%d", op.BN, op.BK, (int)op.head);
-        CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, kSmemBudget + kSmemExtra));
+        CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, kSmemMax));
         CK(launch_k(e->fn, op.grid, kPatchThreads, op.dyn_smem, st, op.pp, pdl));
-        ctx->launches++;
-        return W2L_OK;
-    }
-    if (op.swap) {
-        static uint64_t attr_set[2] = {0, 0};
-        void (*fn)(const ConvParams) = ctx->bf16 ? conv_swap_kernel<true> : conv_swap_kernel<false>;
-        CKR(ensure_smem_attr(&attr_set[ctx->bf16 ? 1 : 0], ctx->device, (const void*)fn, SwapCfg::kSmemBytes));
-        CK(launch_k(fn, op.grid, SwapCfg::kThreads, (size_t)SwapCfg::kSmemBytes, st, op.cp, pdl));
         ctx->launches++;
         return W2L_OK;
     }

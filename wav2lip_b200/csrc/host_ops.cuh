@@ -1,5 +1,5 @@
 // host_ops.cuh — turning one conv block of a spec table into launches: tile/box selection, TMA tensor maps for the
-// activations / weights / outputs, the parameter blocks of the four kernel families, transposed-conv phases.
+// activations / weights / outputs, the parameter blocks of the three kernel families, transposed-conv phases.
 // Part of the single translation unit w2l_api.cu (included there, in this order).
 #pragma once
 
@@ -140,8 +140,7 @@ static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) 
     g->wbytes = w.ntaps * w.cin_pad * a.cout * 2;
     g->stg_bytes = 2 * ((kTileM * a.cout * 2 + 1023) / 1024 * 1024);  // the kernel always carves two staging tiles
     if (g->PW > 256 || g->PH > 256) return false;
-    const int need_stages = a.res ? 3 : 2;  // the epilogue holds the patch of a residual block a little longer
-    if (g->wbytes + g->stg_bytes + need_stages * (w.cin_pad / g->BK) * g->patch_stride > kSmemBudget) return false;
+    if (g->wbytes + g->stg_bytes + 2 * (w.cin_pad / g->BK) * g->patch_stride > kSmemBudget) return false;
     g->res_tap = -1;
     if (a.res) {
         // the patch kernel takes the residual from the input patch in shared memory: it must BE the block input
@@ -174,12 +173,12 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     h.ntaps = w.ntaps;
     h.patch_bytes = g.patch_bytes; h.patch_stride = g.patch_stride;
     for (int t = 0; t < w.ntaps; ++t) h.tap_row[t] = (w.dy[t] - g.oy) * g.PW + (w.dx[t] - g.ox);
-    h.stages = std::min(kPatchMaxStages, (kSmemBudget - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride));
-    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + kSmemExtra;
-    if (op.dyn_smem > kSmemBudget + kSmemExtra || h.stages < 2) return fail(W2L_EINVAL, "%s: patch kernel smem plan %d B / %d stages", a.name.c_str(), op.dyn_smem, h.stages);
+    // even: the two consumer warpgroups take alternate tiles, so each stage always goes to the same one
+    h.stages = std::min(kPatchMaxStages, (kSmemBudget - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride)) & ~1;
+    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + 2 * xbuf_bytes<32>() + kSmemExtra;
+    if (op.dyn_smem > kSmemMax || h.stages < 2) return fail(W2L_EINVAL, "%s: patch kernel smem plan %d B / %d stages", a.name.c_str(), op.dyn_smem, h.stages);
     fill_epi(&h.ep, a);
     h.res_row = g.res_tap >= 0 ? h.tap_row[g.res_tap] : -1;
-    h.pair = h.stages >= 3 ? 1 : 0;  // two tiles in flight + at least one being prefetched
     if (!a.head) {
         // TMA-store view of the output: the BN-channel slice, with this launch's pixel strides (transposed-conv phases
         // interleave), box = one 8 x 16 tile; out-of-range pixels of ragged tiles are clipped by the TMA unit
@@ -212,100 +211,11 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     return W2L_OK;
 }
 
-// The narrowest 96 x 96 layers: S output rows per GEMM row (conv_rowstack.cuh).  Returns the shape id or -1.
-static int rowstack_eligible(const w2l_ctx* ctx, const ConvArgs& a, int* tap_of) {
-    if (!ctx->use_rowstack || !ctx->use_patch || ctx->x2) return -1;
-    const PackedW& w = *a.w;
-    if (a.sx != 1 || a.sy != 1 || a.osx != 1 || a.osy != 1 || a.out.f32 || a.res) return -1;
-    int shape = -1;
-    if (a.head && a.cout == 32 && w.cin_pad == 80 && w.cout_pad == 32 && w.ntaps == 9 && !w.fold && !a.in.nwin && a.in.wstride == 1) shape = 0;
-    if (!a.head && a.cout == 16 && w.cout_pad == 16 && w.fold && w.ntaps == 7 && w.cin_pad == 64 && a.in.wstride == 1) shape = 1;
-    if (!a.head && a.cout == 32 && w.cout_pad == 32 && w.fold && w.ntaps == 7 && w.cin_pad == 64 && a.in.wstride == 1) shape = 2;
-    if (shape < 0) return -1;
-    const RsShape sh = rs_shape(shape);
-    const int tile_h = sh.tile_h, R = sh.R, ndx = sh.ndx, ty = 2 * R + 1;
-    if (a.Wl % kRsTileW != 0 || a.Hl % tile_h != 0) return -1;   // 96 x 96 here; ragged tiles would waste the pipe
-    // no batch-size threshold: the kernel choice (and with it the fp32 summation order) must not depend on N, so that a
-    // crop's result is bit-identical whatever batch it travels in (tests/test_gpu_nets.py)
-    for (int i = 0; i < ndx * ty; ++i) tap_of[i] = -1;
-    for (int t = 0; t < w.ntaps; ++t) {
-        const int dx = w.dx[t], dy = w.dy[t];
-        if (dy < -R || dy > R || (ndx == 1 ? dx != 0 : (dx < -1 || dx > 1))) return -1;
-        tap_of[(ndx == 1 ? 0 : dx + 1) * ty + (R - dy)] = t;
-    }
-    for (int i = 0; i < ndx * ty; ++i) if (tap_of[i] < 0) return -1;
-    return shape;
-}
-
-static int make_rowstack_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, int shape, const int* tap_of) {
-    Op op;
-    op.type = OP_CONV;
-    op.name = a.name + (shape == 0 ? " [rowstack x2]" : " [fold+rowstack x3]");
-    const RsShape sh = rs_shape(shape);
-    op.rowstack = true;
-    op.rs_shape = shape;
-    op.head = a.head;
-    const PackedW& w = *a.w;
-    const int C = a.cout;
-    op.BN = C; op.BK = 64;
-    RowStackParams& h = op.rs;
-    memset(&h, 0, sizeof(h));
-    const int PW = sh.PW, PH = sh.PH, tile_h = sh.tile_h;
-    CKR(encode_act_map(ctx, &h.tmA0, a.in, 64, PW, PH, 1, 1, 1, a.name.c_str()));
-    CKR(encode_w_map(ctx, &h.tmB0, w, 64, C, a.name.c_str()));
-    if (shape == 0) {
-        CKR(encode_act_map(ctx, &h.tmA1, a.in, 16, PW, PH, 1, 1, 1, a.name.c_str()));
-        CKR(encode_w_map(ctx, &h.tmB1, w, 16, C, a.name.c_str()));
-    } else {
-        h.tmA1 = h.tmA0; h.tmB1 = h.tmB0;
-    }
-    h.tiles_x = a.Wl / kRsTileW;
-    h.tiles_y = a.Hl / tile_h;
-    h.ox = shape == 0 ? -1 : 0;   // folded inputs: the window already starts at the leftmost tap
-    h.oy = -sh.R;
-    for (int i = 0; i < sh.ndx * (2 * sh.R + 1); ++i) h.tap_of[i] = tap_of[i];
-    const int fixed = sh.fixed, per_stage = sh.per_stage;
-    h.stages = std::min(kRsMaxStages, (kSmemBudget + kSmemExtra - fixed) / per_stage);
-    op.dyn_smem = fixed + h.stages * per_stage;
-    if (h.stages < 2) return fail(W2L_EINVAL, "%s: row-stack kernel smem plan %d B / %d stages", a.name.c_str(), op.dyn_smem, h.stages);
-    fill_epi(&h.ep, a);
-    if (!a.head) {
-        EncodeTiledFn enc = get_encode_fn();
-        const CUtensorMapDataType dt = ctx->bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-        const CUtensorMapSwizzle sw = C == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : C == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-        cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)a.Wl, (cuuint64_t)a.Hl, (cuuint64_t)a.in.N};
-        cuuint64_t strides[3] = {(cuuint64_t)h.ep.out_sx * 2, (cuuint64_t)h.ep.out_sy * 2, (cuuint64_t)h.ep.out_sn * 2};
-        cuuint32_t box[4] = {(cuuint32_t)C, (cuuint32_t)kRsTileW, (cuuint32_t)tile_h, 1};
-        cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&h.tmO, dt, 4, h.ep.out, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(W2L_ECUDA, "%s: cuTensorMapEncodeTiled(out) failed with %d", a.name.c_str(), (int)r);
-    } else {
-        h.tmO = h.tmA0;
-    }
-    h.tmO2 = h.tmO;
-    CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(h.cscale, a.scale + a.ch_off, (size_t)C * 4, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(h.cshift, a.shift + a.ch_off, (size_t)C * 4, cudaMemcpyDeviceToHost));
-    if (a.head) {
-        CK(cudaMemcpy(h.chead_w, a.head_w, 96 * 4, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(h.chead_b, a.head_b, 3 * 4, cudaMemcpyDeviceToHost));
-    }
-    const long long total = (long long)h.tiles_x * h.tiles_y * a.in.N;
-    op.grid = (int)std::min<long long>(total, ctx->num_sms);
-    op.flops = 2.0 * a.macs_per_pixel * (double)a.Wl * a.Hl * a.in.N;
-    pl->ops.push_back(op);
-    return W2L_OK;
-}
-
 static int make_conv_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a) {
     if (!get_encode_fn()) return fail(W2L_ENODEV, "cuTensorMapEncodeTiled is not available (no CUDA driver?)");
     const PackedW& w = *a.w;
     if (a.in.C != w.cin_pad) return fail(W2L_EINVAL, "%s: input view has %d channels, weights packed for %d", a.name.c_str(), a.in.C, w.cin_pad);
     if (a.cout % 16 != 0) return fail(W2L_EINVAL, "%s: cout %d not a multiple of 16", a.name.c_str(), a.cout);
-    int rs_taps[21];
-    const int rs_shape = rowstack_eligible(ctx, a, rs_taps);
-    if (rs_shape >= 0) return make_rowstack_op(ctx, pl, a, rs_shape, rs_taps);
     PatchGeom geom;
     if (patch_eligible(ctx, a, &geom)) return make_patch_op(ctx, pl, a, geom);
     Op op;
@@ -319,36 +229,17 @@ static int make_conv_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a) {
     int BN = 16;
     for (int cand : {128, 64, 32, 16})
         if (a.cout % cand == 0) { BN = cand; break; }
-    // 256-wide tiles halve the A-operand traffic (L2 -> smem and smem -> tensor core) per FLOP; worth it once
-    // there are enough tiles to fill the machine several times over
-    if (ctx->use_bn256 && BK == 64 && a.cout % 256 == 0 && (long long)m_tiles * (a.cout / 256) >= 3LL * ctx->num_sms) BN = 256;
     if (a.head) BN = 32;
     else
         while (BN > 32 && m_tiles * (a.cout / BN) < ctx->num_sms && a.cout % (BN / 2) == 0) BN /= 2;
-    // Few-tile layers (<= 6x6 maps at 512 channels): units are dealt round-robin to one CTA per SM, so what counts is
-    // rounds x time per unit.  A K step of one unit costs ~137 cycles at N = 256, ~91 at N = 128, ~68 at N <= 64 (the
-    // operand-path model of DESIGN.md section 3): 90 units of 256 channels in ONE round beat 180 units of 128 in two.
-    // (only with a deep K loop, >= 36 steps: short ones are dominated by the 4-pass epilogue of the wide tile; measured
-    //  profiles/r2_rounds_ab_*: 512-channel 3x3 blocks at 3x3 57 -> 48 us, 4-tap phase 52 -> 44, 1- and 2-tap phases +2..3)
-    if (!a.head && ctx->use_bn256 && ctx->use_rounds && BK == 64 && BN < 256 && a.cout % 256 == 0 && w.cout_pad % 256 == 0 &&
-        w.ntaps * (w.cin_pad / BK) >= 36) {
-        auto rounds = [&](long long units) { return (units + ctx->num_sms - 1) / ctx->num_sms; };
-        const long long cost_cur = rounds((long long)m_tiles * (a.cout / BN)) * (BN == 128 ? 91 : 68);
-        const long long cost_256 = rounds((long long)m_tiles * (a.cout / 256)) * 137;
-        const bool mt2_ahead = ctx->use_mt2 && (long long)((m_tiles + 1) / 2) * (a.cout / BN) >= 2LL * ctx->num_sms;   // handled below
-        if (!mt2_ahead && cost_256 < cost_cur) BN = 256;
-    }
     if (w.cout_pad % BN != 0) return fail(W2L_EINVAL, "%s: cout_pad %d vs BN %d", a.name.c_str(), w.cout_pad, BN);
     op.BN = BN; op.BK = BK; op.head = a.head;
-    // two M tiles per CTA (shared weight slab, two accumulators) once there is plenty of work
+    // two M tiles per CTA (shared weight slab, one consumer warpgroup each) once there is plenty of work
     const int n_tiles_ = a.cout / BN;
     if (ctx->use_mt2 && !a.head && find_conv_kernel(BN, BK, ctx->bf16, false, 2) &&
         (long long)((m_tiles + 1) / 2) * n_tiles_ >= 2LL * ctx->num_sms)
         op.MT = 2;
-    // 128-channel tiles with two pixel tiles per unit: one M=128(channels) x N=256(pixels) instruction per K step instead of
-    // two N=128 ones (conv_swap.cuh: 96 instead of 128 B/clk of shared-memory operand reads)
-    if (ctx->use_swap && ctx->use_tma_epi && op.MT == 2 && BN == 128 && BK == 64 && !ctx->x2 && !a.out.f32) op.swap = true;
-    if (op.MT == 2) op.name += op.swap ? " [swap]" : " [2M]";
+    if (op.MT == 2) op.name += " [2M]";
 
     ConvParams& p = op.cp;
     memset(&p, 0, sizeof(p));
@@ -452,7 +343,7 @@ static int make_convt_fused_op(w2l_ctx* ctx, Plan* pl, const Layer& L, const Lay
     t.patch_bytes = kCtPW * kCtPH * BK * 2;
     t.patch_stride = (t.patch_bytes + 1023) / 1024 * 1024;
     const int stage_bytes = t.patch_stride + 9 * kCtBN * BK * 2;
-    const int fixed = 2 * kTileM * kCtBN * 2 + kSmemExtra;
+    const int fixed = 2 * kTileM * kCtBN * 2 + 2 * xbuf_bytes<16>() + kSmemExtra;
     t.stages = std::min(kCtMaxStages, (kCtSmemMax - fixed) / stage_bytes);
     if (t.stages < 2) return fail(W2L_EINVAL, "%s: fused convT does not fit shared memory", L.name.c_str());
     op.dyn_smem = t.stages * stage_bytes + fixed;

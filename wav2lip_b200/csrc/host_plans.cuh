@@ -111,7 +111,7 @@ static int build_generator_plan(w2l_ctx* ctx, Plan* pl) {
             // TMA store of the same staged tile), read through the overlapping-window map with the 3 horizontal taps
             // folded into K.
             Op& prev = pl->ops.back();
-            if ((!prev.patch && !prev.rowstack) || prev.head) return fail(W2L_ESTATE, "folded stride-2 block needs the patch kernel on the first block");
+            if (!prev.patch || prev.head) return fail(W2L_ESTATE, "folded stride-2 block needs the patch kernel on the first block");
             const Layer& L1 = g.layers[g.face_enc[1][0]];
             Act e0;
             CKR(plan_input_act(pl, &e0, N, 96, 96, L1.cin, nw.layers[g.face_enc[1][0]], L1));
@@ -119,13 +119,12 @@ static int build_generator_plan(w2l_ctx* ctx, Plan* pl) {
             const CUtensorMapDataType dt = ctx->bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
             cuuint64_t od[4] = {16, 96, 96, (cuuint64_t)N};
             cuuint64_t os[3] = {(cuuint64_t)e0.Cs * 2, (cuuint64_t)e0.Wp * e0.Cs * 2, (cuuint64_t)96 * e0.Wp * e0.Cs * 2};
-            cuuint32_t ob[4] = {16, (cuuint32_t)kPatchTileW, (cuuint32_t)(prev.rowstack ? RsCfg1::kTileH : kPatchTileH), 1};
+            cuuint32_t ob[4] = {16, (cuuint32_t)kPatchTileW, (cuuint32_t)kPatchTileH, 1};
             cuuint32_t oe[4] = {1, 1, 1, 1};
-            CUresult r = enc(prev.rowstack ? &prev.rs.tmO2 : &prev.pp.tmO2, dt, 4, e0.base + (size_t)e0.x_off * e0.Cs, od, os, ob, oe, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CUresult r = enc(&prev.pp.tmO2, dt, 4, e0.base + (size_t)e0.x_off * e0.Cs, od, os, ob, oe, CU_TENSOR_MAP_INTERLEAVE_NONE,
                              CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
             if (r != CUDA_SUCCESS) return fail(W2L_ECUDA, "cuTensorMapEncodeTiled(dense copy) failed with %d", (int)r);
             prev.pp.has_out2 = 1;
-            prev.rs.has_out2 = 1;
             x = e0;
         }
     }
@@ -364,8 +363,8 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
             }
             case OP_CONV: {
                 if (op.head) {
-                    op.cp.ep.head_out = u8 ? nullptr : (float*)out0; op.pp.ep.head_out = op.cp.ep.head_out; op.rs.ep.head_out = op.cp.ep.head_out;
-                    op.cp.ep.head_out_u8 = u8 ? (unsigned char*)out0 : nullptr; op.pp.ep.head_out_u8 = op.cp.ep.head_out_u8; op.rs.ep.head_out_u8 = op.cp.ep.head_out_u8;
+                    op.cp.ep.head_out = u8 ? nullptr : (float*)out0; op.pp.ep.head_out = op.cp.ep.head_out;
+                    op.cp.ep.head_out_u8 = u8 ? (unsigned char*)out0 : nullptr; op.pp.ep.head_out_u8 = op.cp.ep.head_out_u8;
                 }
                 CKR(launch_conv(ctx, op, st));
                 break;

@@ -55,7 +55,7 @@ struct TrainPlan {
     std::vector<PackParams> pack_jobs;
     std::vector<PackFoldParams> pack_fold_jobs;
     std::vector<FoldJob> fold_jobs;
-    bool allow_fold = false, allow_rowstack = false;   // the context's own switches (the builder turns them off around itself)
+    bool allow_fold = false;   // the context's own switch (the builder turns them off around itself)
     PackParams* pack_dev = nullptr; int *pack_blk_job = nullptr, *pack_blk_first = nullptr; int pack_blocks = 0;   // one-launch repack
     std::vector<TBlock> blocks;    // forward order
     std::vector<size_t> ingest;    // indices of the ingest ops
@@ -230,9 +230,9 @@ typedef void (*WgKernelFn)(const WgradParams);
 struct WgKernelEntry { int BN; bool bf16; WgKernelFn fn; uint64_t attr_set; };
 static WgKernelEntry g_wg_kernels[] = {
     {16, true, wgrad_kernel<16, true>, 0},   {32, true, wgrad_kernel<32, true>, 0},   {64, true, wgrad_kernel<64, true>, 0},
-    {128, true, wgrad_kernel<128, true>, 0}, {256, true, wgrad_kernel<256, true>, 0},
+    {128, true, wgrad_kernel<128, true>, 0},
     {16, false, wgrad_kernel<16, false>, 0}, {32, false, wgrad_kernel<32, false>, 0}, {64, false, wgrad_kernel<64, false>, 0},
-    {128, false, wgrad_kernel<128, false>, 0}, {256, false, wgrad_kernel<256, false>, 0},
+    {128, false, wgrad_kernel<128, false>, 0},
 };
 constexpr int kWgSmemMax = 225 * 1024;
 
@@ -254,13 +254,13 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     WgradOp& w = b->wg;
     w.on = true;
     const int cn_pad = Tt.C;                 // channels of the view (first layers: padded to 16)
-    int BN = cn_pad <= 16 ? 16 : cn_pad <= 32 ? 32 : cn_pad <= 64 ? 64 : cn_pad <= 128 ? 128 : (cn_pad % 256 == 0 ? 256 : 128);
+    int BN = cn_pad <= 16 ? 16 : cn_pad <= 32 ? 32 : cn_pad <= 64 ? 64 : 128;
     w.BN = BN;
     WgradParams& p = w.wp;
     memset(&p, 0, sizeof(p));
     p.ntaps = folded ? L.kh : L.kh * L.kw;
     if (p.ntaps > kWgMaxTaps) return fail(W2L_EINVAL, "%s: too many taps for wgrad", L.name.c_str());
-    const int max_tg = kWgTmemCols / BN;
+    const int max_tg = kWgMaxCols / BN;
     p.ngroups = (p.ntaps + max_tg - 1) / max_tg;
     p.tg = (p.ntaps + p.ngroups - 1) / p.ngroups;
     p.ngroups = (p.ntaps + p.tg - 1) / p.tg;
@@ -275,7 +275,7 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     }
     p.sx = L.sw; p.sy = L.sh;
     // pixels per chunk: at least three pipeline stages must fit
-    int maxP = (kWgSmemMax - 1024) / 3 / (256 + p.tg * BN * 2) / 16 * 16;
+    int maxP = (kWgSmemMax - xbuf_bytes<16>()) / 3 / (256 + p.tg * BN * 2) / 16 * 16;
     maxP = std::max(16, std::min(128, maxP));
     pick_kbox(S.W, S.H, S.N, p.sx, p.sy, maxP, &p.bw, &p.bh, &p.bn);
     p.P = p.bw * p.bh * p.bn;
@@ -286,9 +286,9 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     p.a_bytes = (unsigned)(2 * p.P * 128);
     p.tap_bytes = (unsigned)(p.P * BN * 2);
     p.stage_bytes = (p.a_bytes + p.tg * p.tap_bytes + 1023u) / 1024u * 1024u;
-    p.stages = std::min(8, (int)((kWgSmemMax - 1024) / p.stage_bytes));
+    p.stages = std::min(8, (int)((kWgSmemMax - xbuf_bytes<16>()) / p.stage_bytes));
     if (p.stages < 2) return fail(W2L_EINVAL, "%s: wgrad stage of %u bytes does not pipeline", L.name.c_str(), p.stage_bytes);
-    w.smem = p.stages * p.stage_bytes + 2048;
+    w.smem = p.stages * p.stage_bytes + xbuf_bytes<16>() + 2048;
     // split K so that about two waves of units exist, each with enough chunks to amortise the pipeline fill
     const long long base_units = (long long)p.m_tiles * p.n_tiles * p.ngroups;
     // (rounded DOWN: units are dealt round-robin to one persistent CTA per SM, so 2 * SMs + 1 units would cost three rounds)
@@ -358,7 +358,7 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
     if ((int)tp->wf.layers.size() <= li) { tp->wf.layers.resize(li + 1); tp->wd.layers.resize(li + 1); }
     ctx->pack_rec = &tp->pack_jobs; ctx->fold_rec = &tp->fold_jobs; ctx->pack_fold_rec = &tp->pack_fold_jobs;
     const bool use_fold_fwd = fold && fold->on && tp->allow_fold && !dx.base;
-    if (use_fold_fwd) { ctx->use_fold = true; ctx->use_rowstack = tp->allow_rowstack; }
+    if (use_fold_fwd) ctx->use_fold = true;
     int r = load_layer(ctx, &tp->wf.layers[li], L, b.W, b.bn ? nullptr : b.b, nullptr, nullptr, nullptr, nullptr, in_hw1, use_fold_fwd, st);
     ctx->pack_fold_rec = nullptr;
     if (r == W2L_OK && dx.base) {
@@ -366,13 +366,13 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
         r = load_dgrad_layer(ctx, &tp->wd.layers[li], L, b.Ld, b.W, st);
     }
     ctx->pack_rec = nullptr; ctx->fold_rec = nullptr;
-    if (r != W2L_OK) { if (use_fold_fwd) { ctx->use_fold = false; ctx->use_rowstack = false; } return r; }
+    if (r != W2L_OK) { if (use_fold_fwd) ctx->use_fold = false; return r; }
     Act conv_out = y;
     if (b.bn) { CKR(tp_act(tp, &b.z, y.N, y.H, y.W, L.cout)); conv_out = b.z; }
     Act x_fwd = x;
     if (use_fold_fwd && tp->wf.layers[li].ph[0].fold) {
         int rr = plan_input_act(&tp->pl, &x_fwd, x.N, x.H, x.W, L.cin, tp->wf.layers[li], L);
-        if (rr != W2L_OK) { ctx->use_fold = false; ctx->use_rowstack = false; return rr; }
+        if (rr != W2L_OK) { ctx->use_fold = false; return rr; }
         add_ingest(&tp->pl, "ingest.fold", fold->src_id, x_fwd, fold->B, fold->C, fold->sB, fold->sC, fold->sT, fold->y_off, fold->Wsrc);
         tp->pl.ops.back().ip.cgrp = fold->cgrp; tp->pl.ops.back().ip.sG = fold->sG;
         tp->ingest.push_back(tp->pl.ops.size() - 1);
@@ -381,7 +381,7 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
     b.fwd0 = tp->pl.ops.size();
     {
         const int rr = emit_block(ctx, &tp->pl, tp->wf, li, L, x_fwd, conv_out, nullptr, false, 1, 1, b.bn ? ACT_NONE : -1);
-        if (use_fold_fwd) { ctx->use_fold = false; ctx->use_rowstack = false; }
+        if (use_fold_fwd) ctx->use_fold = false;
         CKR(rr);
     }
     b.fwd1 = tp->pl.ops.size();
@@ -578,15 +578,15 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
     tp->N = (net == W2L_NET_SYNCNET) ? B : (T > 0 ? B * T : B);
     // the specialised first-layer paths (K-folded input layouts) are inference-only: training keeps plain NHWC inputs,
     // which is what the wgrad kernel reads
-    const bool s_fold = ctx->use_fold, s_rs = ctx->use_rowstack;
-    tp->allow_fold = s_fold && ctx->use_patch; tp->allow_rowstack = s_rs;
-    ctx->use_fold = false; ctx->use_rowstack = false;
+    const bool s_fold = ctx->use_fold;
+    tp->allow_fold = s_fold && ctx->use_patch;
+    ctx->use_fold = false;
     size_t ws_need = 0;
     int r;
     if (net == W2L_NET_GENERATOR) r = build_generator_train_plan(ctx, tp.get(), &ws_need);
     else if (net == W2L_NET_SYNCNET) r = build_syncnet_train_plan(ctx, tp.get(), &ws_need, want_wgrad, input_grad);
     else r = build_disc_train_plan(ctx, tp.get(), &ws_need, want_wgrad, input_grad);
-    ctx->use_fold = s_fold; ctx->use_rowstack = s_rs;
+    ctx->use_fold = s_fold;
     if (r == W2L_OK && ws_need) {
         void* p = nullptr;
         r = plan_alloc(&tp->pl, &p, ws_need);

@@ -127,14 +127,10 @@ struct Op {
     int grid = 0;
     double flops = 0;  // algorithmic (true MACs*2), not padded
     bool patch = false;  // conv_patch_kernel instead of conv_igemm_kernel
-    bool swap = false;   // conv_swap_kernel (M = channels, N = 256 pixels) instead of conv_igemm_kernel<128,64,.,.,2>
     PatchParams pp;
     int dyn_smem = 0;
     bool ctf = false;   // convt_fused_kernel
     ConvTParams tp;
-    bool rowstack = false;  // conv_rowstack_kernel
-    int rs_shape = 0;       // 0: output block (C=32, S=2, 3x3, head)   1: folded 7-row first block (C=16, S=3)
-    RowStackParams rs;
     // ingest
     IngestParams ip;
     int ingest_src = 0;  // which caller tensor: 0 = mel / frames, 1 = face
@@ -173,21 +169,17 @@ struct w2l_ctx {
     int device = 0;
     bool bf16 = false;
     bool x2 = false;        // W2L_PREC_F32X: split fp16 operands (hi + lo), generic kernel only
-    int num_sms = 148;
+    int num_sms = 132;
     bool keep_all = false;  // debug: no buffer reuse, every layer output stays readable
     bool use_patch = true;   // W2L_DISABLE_HALO=1 turns the patch kernel off (A/B testing)
-    bool use_bn256 = true;  // W2L_DISABLE_BN256=1
     bool use_mt2 = true;    // W2L_DISABLE_MT2=1
     bool use_aux_stream = true; // W2L_DISABLE_AUXSTREAM=1: training audio-encoder blocks on the main stream
     bool use_wg_stream = true; // W2L_DISABLE_WGSTREAM=1: training wgrads on the main stream instead of a side stream
-    bool use_rounds = true; // W2L_DISABLE_ROUNDS=1: rounds-based choice of 256-wide tiles for few-tile layers
-    bool use_swap = true;   // W2L_DISABLE_SWAP=1: conv_swap_kernel (channel-major accumulator) for the 128-channel-tile layers
     bool use_tma_epi = true;  // W2L_DISABLE_TMAEPI=1
     bool use_fold_s2 = true;  // W2L_DISABLE_FOLDS2=1
     bool use_ctfused = true;  // W2L_DISABLE_CTFUSED=1
     bool use_fold = true;   // W2L_DISABLE_FOLD=1 / driver rejects overlapping-stride tensor maps
     bool use_pdl = true;      // W2L_DISABLE_PDL=1
-    bool use_rowstack = true;  // W2L_DISABLE_ROWSTACK=1
     bool use_mel_v2 = true;    // W2L_DISABLE_MELV2=1
     NetW nets[4];
     float* s3fd_l2w[3] = {nullptr, nullptr, nullptr};   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)

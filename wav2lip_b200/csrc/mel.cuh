@@ -1,4 +1,4 @@
-// mel.cuh — fused audio.melspectrogram for sm_100a.
+// mel.cuh — fused audio.melspectrogram for sm_90a.
 //
 // One kernel does what /root/reference/audio.py:45-51 does in six NumPy/librosa passes:
 //   pre-emphasis (audio.py:20-23) -> reflect-padded framing + periodic Hann window + 800-point real FFT
@@ -8,7 +8,7 @@
 // Numerics follow the reference's dtypes: pre-emphasis, window and FFT in float64 (scipy.lfilter and
 // the FFT of a float64 frame), spectrum rounded to complex64, magnitude / mel / log / clip in float32.
 // float64 matters: with a loud tone in the frame, a float32 FFT's noise floor (-144 dB re peak) reaches
-// the mel bands near the 1e-5 clipping floor and breaks the 1e-4 tolerance; the B200 has the FP64 rate.
+// the mel bands near the 1e-5 clipping floor and breaks the 1e-4 tolerance; the H100 has the FP64 rate.
 //
 // Work split: a block owns MEL_FPB consecutive frames (so the (80, F) row-major output is written in
 // 16-byte runs), MEL_TPF threads per frame. The real 800-point FFT is a 400-point complex Stockham FFT

@@ -19,16 +19,14 @@
 
 #include "../../include/w2l.h"
 #include "aux_kernels.cuh"
+#include "conv_igemm.cuh"
 #include "conv_patch.cuh"
-#include "conv_rowstack.cuh"
-#include "conv_swap.cuh"
-#include "conv_tcgen05.cuh"
 #include "convt_fused.cuh"
 #include "mel.cuh"
 #include "netspec.h"
 #include "resize.cuh"
 #include "train_kernels.cuh"
-#include "wgrad_tcgen05.cuh"
+#include "wgrad.cuh"
 
 using namespace w2l;
 
@@ -83,7 +81,7 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
     if (precision != W2L_PREC_F16 && precision != W2L_PREC_BF16 && precision != W2L_PREC_F32X) return fail(W2L_EINVAL, "unknown precision %d", precision);
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(W2L_ENODEV, "device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(W2L_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     if (!get_encode_fn()) return fail(W2L_ENODEV, "cuTensorMapEncodeTiled not found in the driver");
     DeviceGuard g(device);
     w2l_ctx* ctx = new w2l_ctx();
@@ -111,15 +109,11 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
         ctx->use_patch = enabled("W2L_DISABLE_HALO");
         ctx->use_fold = enabled("W2L_DISABLE_FOLD");
         ctx->use_fold_s2 = enabled("W2L_DISABLE_FOLDS2");
-        ctx->use_bn256 = enabled("W2L_DISABLE_BN256");
         ctx->use_mt2 = enabled("W2L_DISABLE_MT2");
-        ctx->use_swap = enabled("W2L_DISABLE_SWAP");
-        ctx->use_rounds = enabled("W2L_DISABLE_ROUNDS");
         ctx->use_wg_stream = enabled("W2L_DISABLE_WGSTREAM");
         ctx->use_aux_stream = enabled("W2L_DISABLE_AUXSTREAM");
         ctx->use_tma_epi = enabled("W2L_DISABLE_TMAEPI");
         ctx->use_ctfused = enabled("W2L_DISABLE_CTFUSED");
-        ctx->use_rowstack = enabled("W2L_DISABLE_ROWSTACK");
         ctx->use_side = enabled("W2L_DISABLE_SIDESTREAM");
         ctx->use_pdl = enabled("W2L_DISABLE_PDL");
         ctx->use_mel_v2 = enabled("W2L_DISABLE_MELV2");
@@ -946,8 +940,8 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     }
     TrainPlan tp;
     tp.net = slot; tp.N = N; tp.B = N; tp.T = 0;
-    const bool s_fold = ctx->use_fold, s_rs = ctx->use_rowstack;
-    ctx->use_fold = false; ctx->use_rowstack = false;
+    const bool s_fold = ctx->use_fold;
+    ctx->use_fold = false;
     Act xin, dxin, yv, dyv, none;
     size_t ws_need = 0;
     int r = tp_act(&tp, &xin, N, H, W, round_up(L.cin, 16));
@@ -960,7 +954,7 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
         r = add_train_block(ctx, &tp, slot, 0, L, xin, yv, dyv, dx ? dxin : none, none, dw != nullptr,
                             L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, &ws_need);
     }
-    ctx->use_fold = s_fold; ctx->use_rowstack = s_rs;
+    ctx->use_fold = s_fold;
     if (r == W2L_OK && ws_need) { void* p = nullptr; r = plan_alloc(&tp.pl, &p, ws_need); tp.wg_ws = (float*)p; }
     if (r == W2L_OK) {
         cudaError_t e = cudaDeviceSynchronize();

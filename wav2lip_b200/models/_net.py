@@ -44,7 +44,7 @@ class NativeNet(nn.Module):
     def _device_index(self, ref: torch.Tensor) -> int:
         if not ref.is_cuda:
             raise _lib.W2LError(
-                f"{type(self).__name__} runs on a CUDA (sm_100) device only; got a {ref.device} tensor. "
+                f"{type(self).__name__} runs on a CUDA (sm_90) device only; got a {ref.device} tensor. "
                 "wav2lip_b200 has no CPU fallback.")
         return ref.device.index if ref.device.index is not None else torch.cuda.current_device()
 

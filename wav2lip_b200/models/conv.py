@@ -48,7 +48,7 @@ class _Block(nn.Module):
         if self.training and len(self.conv_block) > 1:
             raise NotImplementedError("training-mode BatchNorm (batch statistics) is not built yet: call .eval()")
         if not x.is_cuda:
-            raise _lib.W2LError("wav2lip_b200 blocks run on a CUDA (sm_100) device only; there is no CPU path")
+            raise _lib.W2LError("wav2lip_b200 blocks run on a CUDA (sm_90) device only; there is no CPU path")
         x = x.contiguous().float()
         conv = self.conv_block[0]
         bn = self.conv_block[1] if len(self.conv_block) > 1 else None

@@ -79,7 +79,7 @@ class _Binding:
 
 def binding_of(module, ref: torch.Tensor) -> _Binding:
     if not ref.is_cuda:
-        raise _lib.W2LError(f"{type(module).__name__} trains on a CUDA (sm_100) device only; got a {ref.device} tensor")
+        raise _lib.W2LError(f"{type(module).__name__} trains on a CUDA (sm_90) device only; got a {ref.device} tensor")
     idx = ref.device.index if ref.device.index is not None else torch.cuda.current_device()
     b = module.__dict__.get("_w2l_binding")
     if b is None or b.device.index != idx:
