@@ -218,6 +218,22 @@ int w2l_set_debug(w2l_ctx* ctx, int keep_all_layer_outputs);
 /* the kernel's own (80 x 401) Slaney mel filterbank, dense fp32, written to HOST memory */
 int w2l_mel_basis_host(float* out_host);
 
+/* Which conv kernel a launch uses, so that a parity test can assert the path it exercises. */
+#define W2L_KFAM_IGEMM        0   /* generic implicit-GEMM kernel (conv_igemm.cuh) */
+#define W2L_KFAM_PATCH        1   /* patch kernel with resident weights (conv_patch.cuh) */
+#define W2L_KFAM_CONVT_FUSED  2   /* fused 4-phase transposed conv (convt_fused.cuh) */
+typedef struct w2l_kernel_info {
+    char    name[64];   /* the op's plan label ("b [patch]", "b.ph01 [2M]", ...); empty in the table listing */
+    int32_t family;     /* W2L_KFAM_* */
+    int32_t bn, bk, mt, head, bf16, x2, tma_epi, fold;
+    int32_t m_tiles, n_tiles, grid;
+} w2l_kernel_info;
+/* every compiled conv kernel instantiation (generic, patch, fused transposed conv); host only */
+int w2l_debug_kernel_table(int cap, w2l_kernel_info* out);
+/* the conv launches of the last plan of `net`; net = -1: of the last w2l_conv_block_forward call */
+int w2l_debug_plan_kernels(w2l_ctx* ctx, int net, int cap, w2l_kernel_info* out);
+/* Both return the number of entries written (at most cap), or a negative W2L_E* code; out == NULL returns the count. */
+
 /* ---- training step (scope row f1): wav2lip_train.py:210-231, color_syncnet_train.py:146-163, hq_wav2lip_train.py:213-255 ----
  * Train-mode forward (BatchNorm on batch statistics over the T*B flatten, conv.py:8-11 / wav2lip.py:93-94; running
  * averages updated with momentum 0.1) and backward through every block, as kernels: conv / dgrad on the wgmma conv

@@ -24,7 +24,7 @@ CASES = [
     ("gen 3x3 32 res (64B swizzle)", "c", 32, 32, 3, 1, 1, 0, True, 2, 48, 48),
     ("gen 16->32 s2 (32B swizzle)", "c", 16, 32, 3, 2, 1, 0, False, 2, 96, 96),
     ("gen 7x7 6->16", "c", 6, 16, 7, 1, 3, 0, False, 2, 96, 96),
-    ("gen 7x7 6->16 N=5 (row-stack kernel)", "c", 6, 16, 7, 1, 3, 0, False, 5, 96, 96),
+    ("gen 7x7 6->16 N=5", "c", 6, 16, 7, 1, 3, 0, False, 5, 96, 96),
     ("gen 3x3 128 res", "c", 128, 128, 3, 1, 1, 0, True, 3, 12, 12),
     ("gen 3x3 256 res", "c", 256, 256, 3, 1, 1, 0, True, 3, 6, 6),
     ("gen 3x3 384 res", "c", 384, 384, 3, 1, 1, 0, True, 2, 12, 12),
@@ -47,7 +47,7 @@ CASES = [
     ("sync 46x47 s2 -> 23x24", "c", 64, 128, 3, 2, 1, 0, False, 2, 46, 47),
     ("sync 23x24 res", "c", 128, 128, 3, 1, 1, 0, True, 2, 23, 24),
     ("disc 7x7 3->32 lrelu", "n", 3, 32, 7, 1, 3, 0, False, 2, 48, 96),
-    ("disc 7x7 3->32 lrelu N=9 (row-stack kernel)", "n", 3, 32, 7, 1, 3, 0, False, 9, 48, 96),
+    ("disc 7x7 3->32 lrelu N=9", "n", 3, 32, 7, 1, 3, 0, False, 9, 48, 96),
     ("disc k5 s(1,2)", "n", 32, 64, 5, (1, 2), 2, 0, False, 2, 48, 96),
     ("disc k5", "n", 64, 64, 5, 1, 2, 0, False, 2, 48, 48),
     ("disc k5 s2", "n", 128, 256, 5, 2, 2, 0, False, 2, 24, 24),
@@ -57,13 +57,13 @@ CASES = [
     ("ragged 5x7", "c", 64, 64, 3, 1, 1, 0, True, 3, 5, 7),
     ("ragged 13x11 s2", "c", 32, 64, 3, 2, 1, 0, False, 5, 13, 11),
     ("N=131 3x3 spatial", "c", 64, 64, 3, 1, 1, 0, True, 131, 3, 3),
-    # batches large enough for many 128-row tiles per SM at 128-channel tiles (the ids keep the names of a retired variant):
+    # batches large enough for many 128-row tiles per SM at 128-channel tiles:
     # residual, three channel tiles, ragged boxes, strided, transposed-conv phases
-    ("swap 3x3 128 res 24x24 N=140", "c", 128, 128, 3, 1, 1, 0, True, 140, 24, 24),
-    ("swap 3x3 384 res 12x12 N=190", "c", 384, 384, 3, 1, 1, 0, True, 190, 12, 12),
-    ("swap ragged 23x24 128 res N=150", "c", 128, 128, 3, 1, 1, 0, True, 150, 23, 24),
-    ("swap 64->128 s2 48x48 N=140", "c", 64, 128, 3, 2, 1, 0, False, 140, 48, 48),
-    ("swap convT s2 320->128 N=150", "t", 320, 128, 3, 2, 1, 1, False, 150, 24, 24),
+    ("large N 3x3 128 res 24x24 N=140", "c", 128, 128, 3, 1, 1, 0, True, 140, 24, 24),
+    ("large N 3x3 384 res 12x12 N=190", "c", 384, 384, 3, 1, 1, 0, True, 190, 12, 12),
+    ("large N ragged 23x24 128 res N=150", "c", 128, 128, 3, 1, 1, 0, True, 150, 23, 24),
+    ("large N 64->128 s2 48x48 N=140", "c", 64, 128, 3, 2, 1, 0, False, 140, 48, 48),
+    ("large N convT s2 320->128 N=150", "t", 320, 128, 3, 2, 1, 1, False, 150, 24, 24),
 ]
 
 

@@ -32,7 +32,9 @@ EXPORTS = [
     "w2l_crop_resize_u8", "w2l_paste_u8", "w2l_lipsync_frames_u8", "w2l_s3fd_out_dims", "w2l_s3fd_forward",
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
+    "w2l_debug_kernel_table", "w2l_debug_plan_kernels",
 ]
+KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
 
 
 class W2LError(RuntimeError):
@@ -43,6 +45,34 @@ class LayerInfo(C.Structure):
     _fields_ = [("name", C.c_char * 64), ("kind", C.c_int32), ("cin", C.c_int32), ("cout", C.c_int32),
                 ("kh", C.c_int32), ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32),
                 ("ph", C.c_int32), ("pw", C.c_int32), ("out_pad", C.c_int32), ("residual", C.c_int32), ("cout_real", C.c_int32)]
+
+
+class KernelInfo(C.Structure):
+    _fields_ = [("name", C.c_char * 64), ("family", C.c_int32), ("bn", C.c_int32), ("bk", C.c_int32), ("mt", C.c_int32),
+                ("head", C.c_int32), ("bf16", C.c_int32), ("x2", C.c_int32), ("tma_epi", C.c_int32), ("fold", C.c_int32),
+                ("m_tiles", C.c_int32), ("n_tiles", C.c_int32), ("grid", C.c_int32)]
+
+    def as_dict(self) -> dict:
+        d = {f: getattr(self, f) for f, _ in self._fields_}
+        d["name"] = self.name.decode()
+        return d
+
+
+def _kernel_rows(fn) -> list:
+    n = fn(0, None)
+    if n < 0:
+        check(n)
+    buf = (KernelInfo * max(n, 1))()
+    k = fn(n, buf)
+    if k < 0:
+        check(k)
+    return [buf[i].as_dict() for i in range(k)]
+
+
+def kernel_table() -> list:
+    """Every compiled conv kernel instantiation as a list of dicts (host only, no GPU needed)."""
+    lib = get_lib()
+    return _kernel_rows(lambda cap, out: lib.w2l_debug_kernel_table(cap, out))
 
 
 def lib_path() -> str:
@@ -117,6 +147,8 @@ def get_lib() -> C.CDLL:
     lib.w2l_comm_unique_id.argtypes = [vp, C.c_char_p]
     lib.w2l_comm_init.argtypes = [vp, C.c_char_p, i32, i32]
     lib.w2l_conv_block_train.argtypes = [vp, C.POINTER(LayerInfo), vp, i32, i32, i32] + [vp] * 14
+    lib.w2l_debug_kernel_table.argtypes = [i32, C.POINTER(KernelInfo)]
+    lib.w2l_debug_plan_kernels.argtypes = [vp, i32, i32, C.POINTER(KernelInfo)]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here == header / library mismatch
     if lib.w2l_abi_version() != 1:
@@ -182,6 +214,10 @@ class Context:
 
     def set_debug(self, keep_all: bool):
         check(self.lib.w2l_set_debug(self.h, 1 if keep_all else 0))
+
+    def plan_kernels(self, net: int) -> list:
+        """The conv launches of the last plan of `net` (-1: of the last w2l_conv_block_forward) as a list of dicts."""
+        return _kernel_rows(lambda cap, out: self.lib.w2l_debug_plan_kernels(self.h, int(net), cap, out))
 
     def load_weights(self, net: int, tensors: dict, stream: int = 0):
         """tensors: name -> (device_ptr, numel) of fp32 contiguous CUDA tensors."""

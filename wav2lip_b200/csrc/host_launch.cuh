@@ -54,7 +54,6 @@ typedef void (*CtKernelFn)(const ConvTParams);
 struct CtKernelEntry { int BK; bool bf16; CtKernelFn fn; uint64_t attr_set; };
 static CtKernelEntry g_ct_kernels[] = {
     {32, false, convt_fused_kernel<32, false>, 0}, {32, true, convt_fused_kernel<32, true>, 0},
-    {64, false, convt_fused_kernel<64, false>, 0}, {64, true, convt_fused_kernel<64, true>, 0},
 };
 constexpr int kCtSmemMax = 227 * 1024;
 
@@ -84,6 +83,18 @@ static cudaError_t launch_k(void (*fn)(const P), int grid, int block, size_t sme
     cfg.attrs = at;
     cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, fn, p);
+}
+
+// the w2l_kernel_info row of one conv Op (test aid: which kernel instantiation the launch uses)
+static void op_kernel_info(const w2l_ctx* ctx, const Op& op, w2l_kernel_info* k) {
+    memset(k, 0, sizeof(*k));
+    snprintf(k->name, sizeof(k->name), "%s", op.name.c_str());
+    k->family = op.ctf ? W2L_KFAM_CONVT_FUSED : op.patch ? W2L_KFAM_PATCH : W2L_KFAM_IGEMM;
+    k->bn = op.BN; k->bk = op.BK; k->mt = op.MT; k->head = op.head ? 1 : 0;
+    k->bf16 = ctx->bf16 ? 1 : 0; k->x2 = ctx->x2 ? 1 : 0;
+    k->tma_epi = (!op.ctf && !op.patch && op.cp.tma_epi) ? 1 : 0;
+    k->fold = op.fold ? 1 : 0;
+    k->m_tiles = op.m_tiles; k->n_tiles = op.n_tiles; k->grid = op.grid;
 }
 
 static int launch_conv(w2l_ctx* ctx, const Op& op, cudaStream_t st, bool pdl = true) {

@@ -206,6 +206,7 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     }
     const long long total = (long long)h.tiles_x * h.tiles_y * a.in.N;
     op.grid = (int)std::min<long long>(total, ctx->num_sms);
+    op.fold = w.fold; op.m_tiles = (int)total; op.n_tiles = 1;
     op.flops = 2.0 * a.macs_per_pixel * (double)a.Wl * a.Hl * a.in.N;
     pl->ops.push_back(op);
     return W2L_OK;
@@ -297,6 +298,7 @@ static int make_conv_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a) {
     }
     const int total = ((m_tiles + op.MT - 1) / op.MT) * p.n_tiles;
     op.grid = std::min(total, ctx->num_sms);
+    op.fold = w.fold; op.m_tiles = m_tiles; op.n_tiles = p.n_tiles;
     op.flops = 2.0 * a.macs_per_pixel * (double)a.Wl * a.Hl * a.in.N;
     pl->ops.push_back(op);
     return W2L_OK;
@@ -311,14 +313,17 @@ static int make_convt_fused_op(w2l_ctx* ctx, Plan* pl, const Layer& L, const Lay
     op.type = OP_CONV;
     op.name = L.name + " [fused 4-phase]";
     op.ctf = true;
-    const int BK = pick_bk(w.cin_pad);
+    // K steps of 32 channels whatever cin is: one 64-channel stage (patch + nine 64x64 weight slabs, 94 KB) would not
+    // double-buffer in shared memory
+    const int BK = 32;
+    if (w.cin_pad % BK != 0) return fail(W2L_EINVAL, "%s: fused convT needs cin %% 32 == 0", L.name.c_str());
     op.BK = BK; op.BN = kCtBN;
     ConvTParams& t = op.tp;
     memset(&t, 0, sizeof(t));
     CKR(encode_act_map(ctx, &t.tmA, in, BK, kCtPW, kCtPH, 1, 1, 1, L.name.c_str()));
     {
         const CUtensorMapDataType dt = ctx->bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-        const CUtensorMapSwizzle sw = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+        const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_64B;  // 64-byte (BK = 32) rows
         cuuint64_t dims[3] = {(cuuint64_t)w.cin_pad, (cuuint64_t)w.cout_pad, 9};
         cuuint64_t strides[2] = {(cuuint64_t)w.cin_pad * 2, (cuuint64_t)w.cin_pad * w.cout_pad * 2};
         cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)kCtBN, 9};
@@ -353,6 +358,7 @@ static int make_convt_fused_op(w2l_ctx* ctx, Plan* pl, const Layer& L, const Lay
     CK(cudaMemcpy(t.cshift, lw.shift, kCtBN * 4, cudaMemcpyDeviceToHost));
     const long long units = (long long)t.tiles_x * t.tiles_y * in.N;
     op.grid = (int)std::min<long long>(units, ctx->num_sms);
+    op.m_tiles = (int)units; op.n_tiles = 1;
     op.flops = 2.0 * (double)L.cin * L.cout * 9 * (double)in.W * in.H * in.N;
     pl->ops.push_back(op);
     return W2L_OK;
@@ -391,7 +397,10 @@ static int emit_block(w2l_ctx* ctx, Plan* pl, const NetW& nw, int li, const Laye
         a.macs_per_pixel = (double)L.cin * L.cout * L.kh * L.kw;
         return make_conv_op(ctx, pl, a);
     }
-    if (lw.has_all_taps && ctx->use_ctfused && in.W >= 8 && in.H >= 8 && !res && out.H == 2 * in.H && out.W == 2 * in.W &&
+    // the fused kernel steps K by 32 channels (g_ct_kernels): a cin that is not a multiple of 32 (16, 48, 80, ...) takes
+    // the four phase launches
+    if (lw.has_all_taps && ctx->use_ctfused && lw.ph.back().cin_pad % 32 == 0 && in.W >= 8 && in.H >= 8 && !res &&
+        out.H == 2 * in.H && out.W == 2 * in.W &&
         (double)in.W * in.H / ((double)((in.W + 7) / 8) * ((in.H + 15) / 16) * kTileM) >= 0.6 && !out.f32)
         return make_convt_fused_op(ctx, pl, L, lw, in, out, a.act);
     const size_t nph = lw.ph.size() - (lw.has_all_taps ? 1 : 0);

@@ -131,6 +131,8 @@ struct Op {
     int dyn_smem = 0;
     bool ctf = false;   // convt_fused_kernel
     ConvTParams tp;
+    bool fold = false;  // K-folded first layer
+    int m_tiles = 0, n_tiles = 0;  // output tiles along pixels / channels (w2l_debug_plan_kernels)
     // ingest
     IngestParams ip;
     int ingest_src = 0;  // which caller tensor: 0 = mel / frames, 1 = face
@@ -185,6 +187,7 @@ struct w2l_ctx {
     float* s3fd_l2w[3] = {nullptr, nullptr, nullptr};   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)
     std::map<std::string, std::unique_ptr<Plan>> plans;
     Plan* last_plan[4] = {nullptr, nullptr, nullptr, nullptr};
+    std::vector<w2l_kernel_info> last_block_kernels;  // conv launches of the last w2l_conv_block_forward (its plan is freed)
     int64_t launches = 0;
     long long plan_clock = 0;
     size_t weight_bytes = 0;

@@ -542,10 +542,13 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float
     Act in, out;
     if (r == W2L_OK) r = plan_input_act(&pl, &in, N, H, W, L.cin, scratch.layers[0], L);
     if (r == W2L_OK) r = plan_act(&pl, &out, N, Ho, Wo, L.cout);
+    ctx->last_block_kernels.clear();
     if (r == W2L_OK) {
         add_ingest(&pl, "ingest.x", 0, in, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W);
         r = emit_block(ctx, &pl, scratch, 0, L, in, out, L.residual ? &in : nullptr);
         if (r == W2L_OK) {
+            for (const Op& op : pl.ops)
+                if (op.type == OP_CONV) { ctx->last_block_kernels.emplace_back(); op_kernel_info(ctx, op, &ctx->last_block_kernels.back()); }
             Plan* lp = ctx->last_plan[W2L_NET_DISC];
             r = run_plan(ctx, &pl, x, nullptr, nullptr, nullptr, st);  // (pl.net only labels the plan)
             ctx->last_plan[W2L_NET_DISC] = lp;
@@ -564,6 +567,40 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float
     free_layer(scratch.layers[0]);
     ctx->use_fold = saved_fold;
     return r;
+}
+
+int w2l_debug_kernel_table(int cap, w2l_kernel_info* out) {
+    std::vector<w2l_kernel_info> t;
+    auto add = [&](int fam, int bn, int bk, int mt, bool head, bool bf16) {
+        w2l_kernel_info k;
+        memset(&k, 0, sizeof(k));
+        k.family = fam; k.bn = bn; k.bk = bk; k.mt = mt; k.head = head ? 1 : 0; k.bf16 = bf16 ? 1 : 0;
+        t.push_back(k);
+    };
+    for (const auto& e : g_conv_kernels) add(W2L_KFAM_IGEMM, e.BN, e.BK, e.mt, e.head, e.bf16);
+    for (const auto& e : g_patch_kernels) add(W2L_KFAM_PATCH, e.BN, e.BK, 1, e.head, e.bf16);
+    for (const auto& e : g_ct_kernels) add(W2L_KFAM_CONVT_FUSED, kCtBN, e.BK, 1, false, e.bf16);
+    if (!out) return (int)t.size();
+    const int k = std::min<int>(std::max(cap, 0), (int)t.size());
+    for (int i = 0; i < k; ++i) out[i] = t[i];
+    return k;
+}
+
+int w2l_debug_plan_kernels(w2l_ctx* ctx, int net, int cap, w2l_kernel_info* out) {
+    if (!ctx || net < -1 || net > 3) return fail(W2L_EINVAL, "bad argument");
+    std::vector<w2l_kernel_info> t;
+    if (net < 0) {
+        t = ctx->last_block_kernels;
+    } else {
+        const Plan* pl = ctx->last_plan[net];
+        if (!pl) return fail(W2L_ESTATE, "no forward has run for net %d", net);
+        for (const Op& op : pl->ops)
+            if (op.type == OP_CONV) { t.emplace_back(); op_kernel_info(ctx, op, &t.back()); }
+    }
+    if (!out) return (int)t.size();
+    const int k = std::min<int>(std::max(cap, 0), (int)t.size());
+    for (int i = 0; i < k; ++i) out[i] = t[i];
+    return k;
 }
 
 int w2l_debug_layer_output(w2l_ctx* ctx, int net, int layer, float* y, int* n, int* c, int* h, int* w, void* stream) {
