@@ -312,6 +312,48 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
  * that trips it must run in W2L_PREC_BF16 (fp32's exponent range).  bf16 contexts never set it. */
 int w2l_f16_overflow(w2l_ctx* ctx, int clear, int* flag, void* stream);
 
+/* ---- training test aids: the blocks of a training plan and their tape, for per-block parity tests ---- */
+#define W2L_WG_PLAIN       0   /* stride-1 conv: dz on the dense pixel grid, x read at the tap offset */
+#define W2L_WG_STRIDED     1   /* strided conv: x read at stride x output pixel + tap offset */
+#define W2L_WG_TRANSPOSED  2   /* transposed conv: x on the dense grid, dz read strided */
+#define W2L_WG_SWAP        3   /* stride-1 conv with wide input, narrow output: x on the dense grid, dz per tap */
+#define W2L_WG_FOLDED      4   /* K-folded first layer: a "tap" is a filter row of the folded input copy */
+typedef struct w2l_train_block_info {
+    char    name[64];            /* the block's state_dict prefix ("block" for w2l_conv_block_train) */
+    int32_t layer;               /* index into the net's table */
+    int32_t kind, cin, cout, kh, kw, sh, sw, ph, pw, out_pad, residual;
+    int32_t n, h_in, w_in, h_out, w_out;
+    int32_t lane;                /* 1: audio-encoder block (runs on the auxiliary stream beside the face encoder) */
+    int32_t has_dx, has_dx_add, has_du, has_wgrad;
+    /* the weight-gradient op (zero when has_wgrad == 0): wgrad_kernel<wg_bn> + the split-K reduction */
+    int32_t wg_bn, wg_form, wg_ntaps, wg_tg, wg_ngroups;
+    int32_t wg_p, wg_bw, wg_bh, wg_bnb;   /* pixels per K chunk = the box wg_bw x wg_bh x wg_bnb images */
+    int32_t wg_chunks, wg_m_tiles, wg_n_tiles, wg_splits, wg_grid;
+    /* the conv launches of the block's forward and of its input gradient (dgrad) */
+    int32_t n_fwd, n_dgrad;
+    w2l_kernel_info fwd[4], dgrad[4];
+} w2l_train_block_info;
+/* The blocks of the last training plan of `net` in forward order; net = -1: the block of the last w2l_conv_block_train.
+ * Returns the number of entries written (at most cap), or a negative W2L_E* code; out == NULL returns the count. */
+int w2l_debug_train_blocks(w2l_ctx* ctx, int net, int cap, w2l_train_block_info* out);
+
+/* One tape tensor of block `block` (forward order) of the last training plan of `net`, as fp32 NCHW with exactly the
+ * stored 16-bit values: X input, Z pre-BatchNorm conv output, Y output, DY its gradient, DZ gradient of Z (of the conv
+ * output), DU gradient of the residual branch, DX input gradient, DX_ADD the skip gradient added to it; STATS is the
+ * batch statistics (n = 2: mean, invstd; c = cout; h = w = 1) in fp32.  *n,*c,*h,*w receive the dims (any may be NULL);
+ * out_dev == NULL only queries them.  A tensor the block does not have is W2L_EINVAL. */
+#define W2L_TAPE_X      0
+#define W2L_TAPE_Z      1
+#define W2L_TAPE_Y      2
+#define W2L_TAPE_DY     3
+#define W2L_TAPE_DZ     4
+#define W2L_TAPE_DU     5
+#define W2L_TAPE_DX     6
+#define W2L_TAPE_DX_ADD 7
+#define W2L_TAPE_STATS  8
+int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* out_dev, int* n, int* c, int* h, int* w,
+                           void* stream);
+
 /* ---- instrumentation ---- */
 /* kernels launched by this library since the context was created (all streams) */
 int64_t w2l_launch_count(const w2l_ctx* ctx);

@@ -32,9 +32,11 @@ EXPORTS = [
     "w2l_crop_resize_u8", "w2l_paste_u8", "w2l_lipsync_frames_u8", "w2l_s3fd_out_dims", "w2l_s3fd_forward",
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
-    "w2l_debug_kernel_table", "w2l_debug_plan_kernels",
+    "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
 ]
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
+WG_PLAIN, WG_STRIDED, WG_TRANSPOSED, WG_SWAP, WG_FOLDED = 0, 1, 2, 3, 4
+TAPE_X, TAPE_Z, TAPE_Y, TAPE_DY, TAPE_DZ, TAPE_DU, TAPE_DX, TAPE_DX_ADD, TAPE_STATS = range(9)
 
 
 class W2LError(RuntimeError):
@@ -55,6 +57,23 @@ class KernelInfo(C.Structure):
     def as_dict(self) -> dict:
         d = {f: getattr(self, f) for f, _ in self._fields_}
         d["name"] = self.name.decode()
+        return d
+
+
+class TrainBlockInfo(C.Structure):
+    _fields_ = ([("name", C.c_char * 64)]
+                + [(f, C.c_int32) for f in (
+                    "layer", "kind", "cin", "cout", "kh", "kw", "sh", "sw", "ph", "pw", "out_pad", "residual",
+                    "n", "h_in", "w_in", "h_out", "w_out", "lane", "has_dx", "has_dx_add", "has_du", "has_wgrad",
+                    "wg_bn", "wg_form", "wg_ntaps", "wg_tg", "wg_ngroups", "wg_p", "wg_bw", "wg_bh", "wg_bnb",
+                    "wg_chunks", "wg_m_tiles", "wg_n_tiles", "wg_splits", "wg_grid", "n_fwd", "n_dgrad")]
+                + [("fwd", KernelInfo * 4), ("dgrad", KernelInfo * 4)])
+
+    def as_dict(self) -> dict:
+        d = {f: getattr(self, f) for f, _ in self._fields_ if f not in ("name", "fwd", "dgrad")}
+        d["name"] = self.name.decode()
+        d["fwd"] = [self.fwd[i].as_dict() for i in range(self.n_fwd)]
+        d["dgrad"] = [self.dgrad[i].as_dict() for i in range(self.n_dgrad)]
         return d
 
 
@@ -149,6 +168,9 @@ def get_lib() -> C.CDLL:
     lib.w2l_conv_block_train.argtypes = [vp, C.POINTER(LayerInfo), vp, i32, i32, i32] + [vp] * 14
     lib.w2l_debug_kernel_table.argtypes = [i32, C.POINTER(KernelInfo)]
     lib.w2l_debug_plan_kernels.argtypes = [vp, i32, i32, C.POINTER(KernelInfo)]
+    lib.w2l_debug_train_blocks.argtypes = [vp, i32, i32, C.POINTER(TrainBlockInfo)]
+    lib.w2l_debug_train_tensor.argtypes = [vp, i32, i32, i32, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
+                                           C.POINTER(i32), vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here == header / library mismatch
     if lib.w2l_abi_version() != 1:
@@ -218,6 +240,32 @@ class Context:
     def plan_kernels(self, net: int) -> list:
         """The conv launches of the last plan of `net` (-1: of the last w2l_conv_block_forward) as a list of dicts."""
         return _kernel_rows(lambda cap, out: self.lib.w2l_debug_plan_kernels(self.h, int(net), cap, out))
+
+    def train_blocks(self, net: int) -> list:
+        """The blocks of the last training plan of `net` (-1: of the last w2l_conv_block_train) as a list of dicts."""
+        n = self.lib.w2l_debug_train_blocks(self.h, int(net), 0, None)
+        if n < 0:
+            check(n)
+        buf = (TrainBlockInfo * max(n, 1))()
+        k = self.lib.w2l_debug_train_blocks(self.h, int(net), n, buf)
+        if k < 0:
+            check(k)
+        return [buf[i].as_dict() for i in range(k)]
+
+    def train_tensor(self, net: int, block: int, which: int, stream: int = 0):
+        """One tape tensor of a block of the last training plan of `net` (TAPE_*) as a float32 CUDA tensor (NCHW; STATS:
+        (2, C, 1, 1) = mean, invstd), or None if the block has no such tensor.  Synchronises `stream`."""
+        import torch
+        d = [C.c_int32() for _ in range(4)]
+        r = self.lib.w2l_debug_train_tensor(self.h, int(net), int(block), int(which), None, *[C.byref(v) for v in d], None)
+        if r == W2L_EINVAL:
+            return None
+        check(r)
+        out = torch.empty(tuple(v.value for v in d), device=f"cuda:{self.device}", dtype=torch.float32)
+        check(self.lib.w2l_debug_train_tensor(self.h, int(net), int(block), int(which), C.c_void_p(out.data_ptr()),
+                                              None, None, None, None, C.c_void_p(stream)))
+        torch.cuda.synchronize(self.device)
+        return out
 
     def load_weights(self, net: int, tensors: dict, stream: int = 0):
         """tensors: name -> (device_ptr, numel) of fp32 contiguous CUDA tensors."""

@@ -15,9 +15,12 @@
 
 struct ParamRef { float* value = nullptr; float* grad = nullptr; long long n = 0; };
 
+enum WgForm { WG_PLAIN = 0, WG_STRIDED = 1, WG_TRANSPOSED = 2, WG_SWAP = 3, WG_FOLDED = 4 };   // = W2L_WG_*
+
 struct WgradOp {
     bool on = false;
     int BN = 0;
+    int form = WG_PLAIN;
     WgradParams wp;
     WgradReduceParams rp;
     int grid = 0, smem = 0;
@@ -67,7 +70,9 @@ struct TrainPlan {
     const float *a_out = nullptr, *v_out = nullptr;
     // disc
     Act feat, dfeat, dframes_in; const float* prob_out = nullptr;
-    float* wg_ws = nullptr; size_t wg_ws_bytes = 0;
+    // split-K workspace of the wgrads, one per lane: with the wgrad side stream off, each block's wgrad runs on its own
+    // lane's stream, and the audio encoder's (auxiliary stream) run concurrently with the face encoder's (main stream)
+    float* wg_ws[2] = {nullptr, nullptr}; size_t wg_ws_bytes[2] = {0, 0};
     bool input_grad = false;       // the first block's dgrad is part of the plan (expert / discriminator inside a generator step)
     double fwd_flops = 0;
 };
@@ -103,6 +108,7 @@ struct TrainState {
     cudaStream_t s_wg = nullptr; cudaEvent_t ev_dz = nullptr, ev_wg = nullptr, ev_wgb = nullptr;
     // the audio encoder (small, latency-bound launches) runs beside the face encoder, forward and backward
     cudaStream_t s_aux = nullptr; cudaEvent_t ev_aux_fork = nullptr, ev_aux_join = nullptr;
+    std::vector<w2l_train_block_info> last_block_info;   // the block of the last w2l_conv_block_train (its plan is freed)
 };
 
 static TrainState* train_state(w2l_ctx* ctx) {
@@ -154,7 +160,8 @@ static int bound_ptr(TrainState* ts, int net, const std::string& name, long long
 }
 
 // The input gradient of a block, written as a block of the same table (oracle/backward_recipe.py: conv_dgrad).
-static Layer dgrad_layer(const Layer& L, int Hin, int Win, int Ho, int Wo) {
+//   widen: the staged (TMA-store) epilogue is on, which can store fewer channels than a launch computes
+static Layer dgrad_layer(const Layer& L, int Hin, int Win, int Ho, int Wo, bool widen) {
     Layer d = L;
     d.residual = false;
     d.cin = L.cout;
@@ -166,8 +173,9 @@ static Layer dgrad_layer(const Layer& L, int Hin, int Win, int Ho, int Wo) {
         d.kind = W2L_BLOCK_CONV_PLAIN;
         d.ph = L.kh - 1 - L.ph; d.pw = L.kw - 1 - L.pw;
         // 80 input channels (the output block) would tile as 5 x 16 output channels, each pass re-reading dz: compute 128
-        // (48 zero rows) in one pass instead; the TMA store clips at the real channel count
-        if (d.cout > 64 && d.cout % 64 != 0 && d.cout < 128) d.cout = 128;
+        // (48 zero rows) in one pass instead; the TMA store clips at the real channel count (the direct epilogue cannot:
+        // with W2L_DISABLE_TMAEPI the plan keeps the real width)
+        if (widen && d.cout > 64 && d.cout % 64 != 0 && d.cout < 128) d.cout = 128;
     } else {                                   // strided conv      ->  transposed conv with the SAME tensor
         d.kind = W2L_BLOCK_CONVT_BN_RELU;
         d.out_pad = Hin - ((Ho - 1) * L.sh - 2 * L.ph + L.kh);   // rows the forward's floor division dropped (per axis: emit uses out dims)
@@ -227,15 +235,13 @@ static void pick_kbox(int W, int H, int N, int sx, int sy, int maxP, int* bw, in
 }
 
 typedef void (*WgKernelFn)(const WgradParams);
-struct WgKernelEntry { int BN; bool bf16; WgKernelFn fn; uint64_t attr_set; };
-static WgKernelEntry g_wg_kernels[] = {
-    {16, true, wgrad_kernel<16, true>, 0},   {32, true, wgrad_kernel<32, true>, 0},   {64, true, wgrad_kernel<64, true>, 0},
-    {128, true, wgrad_kernel<128, true>, 0},
-    {16, false, wgrad_kernel<16, false>, 0}, {32, false, wgrad_kernel<32, false>, 0}, {64, false, wgrad_kernel<64, false>, 0},
-    {128, false, wgrad_kernel<128, false>, 0},
+struct WgKernelEntry { int BN; WgKernelFn fn; uint64_t attr_set; };
+static WgKernelEntry g_wg_kernels[] = {   // bf16 operands only: training refuses fp16 contexts (get_train_plan)
+    {16, wgrad_kernel<16, true>, 0}, {32, wgrad_kernel<32, true>, 0}, {64, wgrad_kernel<64, true>, 0}, {128, wgrad_kernel<128, true>, 0},
 };
 constexpr int kWgSmemMax = 225 * 1024;
 
+// ws_need[lane]: the largest split-K workspace of the lane's blocks
 static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need) {
     const Layer& L = b->L;
     const bool convT = L.kind == W2L_BLOCK_CONVT_BN_RELU;
@@ -256,6 +262,7 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     const int cn_pad = Tt.C;                 // channels of the view (first layers: padded to 16)
     int BN = cn_pad <= 16 ? 16 : cn_pad <= 32 ? 32 : cn_pad <= 64 ? 64 : 128;
     w.BN = BN;
+    w.form = folded ? WG_FOLDED : swap ? WG_SWAP : convT ? WG_TRANSPOSED : (L.sh > 1 || L.sw > 1) ? WG_STRIDED : WG_PLAIN;
     WgradParams& p = w.wp;
     memset(&p, 0, sizeof(p));
     p.ntaps = folded ? L.kh : L.kh * L.kw;
@@ -299,7 +306,7 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     CKR(encode_act_map(ctx, &p.tmS, S, 64, p.bw, p.bh, p.bn, 1, 1, L.name.c_str()));
     CKR(encode_act_map(ctx, &p.tmT, Tt, std::min(BN, 64), p.bw * p.sx, p.bh * p.sy, p.bn, p.sx, p.sy, L.name.c_str()));
     const long long Mp = (long long)p.m_tiles * 128, Np = (long long)p.n_tiles * BN;
-    *ws_need = std::max<size_t>(*ws_need, (size_t)((long long)p.splits * p.ntaps * Mp * Np * 4));
+    ws_need[b->lane] = std::max<size_t>(ws_need[b->lane], (size_t)((long long)p.splits * p.ntaps * Mp * Np * 4));
     w.grid = (int)std::min<long long>(base_units * p.splits, ctx->num_sms);
     WgradReduceParams& r = w.rp;
     r.ws = nullptr; r.out = b->gW; r.splits = p.splits; r.ntaps = p.ntaps; r.Cm = Cm; r.Cn = Cn; r.Mp = Mp; r.Np = Np; r.accumulate = 0;
@@ -311,13 +318,13 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
 
 static int launch_wgrad(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool accumulate, cudaStream_t st) {
     WgKernelEntry* e = nullptr;
-    for (auto& k : g_wg_kernels) if (k.BN == b.wg.BN && k.bf16 == ctx->bf16) e = &k;
+    for (auto& k : g_wg_kernels) if (k.BN == b.wg.BN) e = &k;
     if (!e) return fail(W2L_EINVAL, "no wgrad kernel for BN=%d", b.wg.BN);
     CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, kWgSmemMax + 2048));
-    b.wg.wp.ws = tp->wg_ws;
+    b.wg.wp.ws = tp->wg_ws[b.lane];
     CK(launch_k(e->fn, b.wg.grid, kWgThreads, (size_t)b.wg.smem, st, b.wg.wp, ctx->use_pdl));
     WgradReduceParams rp = b.wg.rp;
-    rp.ws = tp->wg_ws; rp.out = b.gW; rp.accumulate = accumulate ? 1 : 0;
+    rp.ws = tp->wg_ws[b.lane]; rp.out = b.gW; rp.accumulate = accumulate ? 1 : 0;
     const int n_tiles64 = (rp.Cn + 63) / 64;
     wgrad_reduce_kernel<<<dim3((unsigned)n_tiles64, (unsigned)rp.Cm), 256, (size_t)64 * (rp.ntaps + 1) * 4, st>>>(rp);
     ctx->launches += 2;
@@ -362,7 +369,7 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
     int r = load_layer(ctx, &tp->wf.layers[li], L, b.W, b.bn ? nullptr : b.b, nullptr, nullptr, nullptr, nullptr, in_hw1, use_fold_fwd, st);
     ctx->pack_fold_rec = nullptr;
     if (r == W2L_OK && dx.base) {
-        b.Ld = dgrad_layer(L, x.H, x.W, y.H, y.W);
+        b.Ld = dgrad_layer(L, x.H, x.W, y.H, y.W, ctx->use_tma_epi);
         r = load_dgrad_layer(ctx, &tp->wd.layers[li], L, b.Ld, b.W, st);
     }
     ctx->pack_rec = nullptr; ctx->fold_rec = nullptr;
@@ -410,10 +417,35 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
         CKR(emit_block(ctx, &tp->pl, tp->wd, li, b.Ld, b.dz, dx, add ? &add_copy : nullptr, false, 1, 1, ACT_NONE));
         b.dg1 = tp->pl.ops.size();
     }
-    if (want_wgrad) CKR(make_wgrad_op(ctx, tp, &b, ws_need));
     b.lane = starts_with(L.name, "audio_encoder.") ? 1 : 0;
+    if (want_wgrad) CKR(make_wgrad_op(ctx, tp, &b, ws_need));
     tp->blocks.push_back(b);
     return W2L_OK;
+}
+
+// the w2l_train_block_info row of one block (test aid)
+static void train_block_info(const w2l_ctx* ctx, const TrainPlan* tp, const TBlock& b, w2l_train_block_info* o) {
+    memset(o, 0, sizeof(*o));
+    const Layer& L = b.L;
+    snprintf(o->name, sizeof(o->name), "%s", L.name.c_str());
+    o->layer = b.li;
+    o->kind = L.kind; o->cin = L.cin; o->cout = L.cout; o->kh = L.kh; o->kw = L.kw; o->sh = L.sh; o->sw = L.sw;
+    o->ph = L.ph; o->pw = L.pw; o->out_pad = L.out_pad; o->residual = L.residual ? 1 : 0;
+    o->n = b.x.N; o->h_in = b.x.H; o->w_in = b.x.W; o->h_out = b.y.H; o->w_out = b.y.W;
+    o->lane = b.lane;
+    o->has_dx = b.dx.base ? 1 : 0; o->has_dx_add = b.dx_add.base ? 1 : 0; o->has_du = b.du.base ? 1 : 0;
+    o->has_wgrad = b.wg.on ? 1 : 0;
+    if (b.wg.on) {
+        const WgradParams& p = b.wg.wp;
+        o->wg_bn = b.wg.BN; o->wg_form = b.wg.form; o->wg_ntaps = p.ntaps; o->wg_tg = p.tg; o->wg_ngroups = p.ngroups;
+        o->wg_p = p.P; o->wg_bw = p.bw; o->wg_bh = p.bh; o->wg_bnb = p.bn;
+        o->wg_chunks = (int32_t)p.chunks; o->wg_m_tiles = p.m_tiles; o->wg_n_tiles = p.n_tiles; o->wg_splits = p.splits;
+        o->wg_grid = b.wg.grid;
+    }
+    for (size_t i = b.fwd0; i < b.fwd1 && o->n_fwd < 4; ++i)
+        if (tp->pl.ops[i].type == OP_CONV) op_kernel_info(ctx, tp->pl.ops[i], &o->fwd[o->n_fwd++]);
+    for (size_t i = b.dg0; i < b.dg1 && o->n_dgrad < 4; ++i)
+        if (tp->pl.ops[i].type == OP_CONV) op_kernel_info(ctx, tp->pl.ops[i], &o->dgrad[o->n_dgrad++]);
 }
 
 // a straight chain of blocks; value and gradient buffers of the intermediate tensors are dense and owned by the plan
@@ -581,16 +613,17 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
     const bool s_fold = ctx->use_fold;
     tp->allow_fold = s_fold && ctx->use_patch;
     ctx->use_fold = false;
-    size_t ws_need = 0;
+    size_t ws_need[2] = {0, 0};
     int r;
-    if (net == W2L_NET_GENERATOR) r = build_generator_train_plan(ctx, tp.get(), &ws_need);
-    else if (net == W2L_NET_SYNCNET) r = build_syncnet_train_plan(ctx, tp.get(), &ws_need, want_wgrad, input_grad);
-    else r = build_disc_train_plan(ctx, tp.get(), &ws_need, want_wgrad, input_grad);
+    if (net == W2L_NET_GENERATOR) r = build_generator_train_plan(ctx, tp.get(), ws_need);
+    else if (net == W2L_NET_SYNCNET) r = build_syncnet_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
+    else r = build_disc_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
     ctx->use_fold = s_fold;
-    if (r == W2L_OK && ws_need) {
+    for (int lane = 0; lane < 2 && r == W2L_OK; ++lane) {
+        if (!ws_need[lane]) continue;
         void* p = nullptr;
-        r = plan_alloc(&tp->pl, &p, ws_need);
-        tp->wg_ws = (float*)p; tp->wg_ws_bytes = ws_need;
+        r = plan_alloc(&tp->pl, &p, ws_need[lane]);
+        tp->wg_ws[lane] = (float*)p; tp->wg_ws_bytes[lane] = ws_need[lane];
     }
     if (r != W2L_OK) { free_train_plan(tp.get()); return r; }
     CK(cudaDeviceSynchronize());
@@ -600,7 +633,7 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// replay
+// replay (training plans exist only on bf16 contexts, get_train_plan: every launch below is the bf16 instantiation)
 // ------------------------------------------------------------------------------------------------
 static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
     if (!tp->pack_jobs.empty()) {
@@ -621,15 +654,13 @@ static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
             CK(cudaMemcpy(tp->pack_blk_first, blk_first.data(), blk_first.size() * 4, cudaMemcpyHostToDevice));
             tp->pack_blocks = (int)blk_job.size();
         }
-        if (ctx->bf16) pack_multi_kernel<true><<<tp->pack_blocks, 256, 0, st>>>(tp->pack_dev, tp->pack_blk_job, tp->pack_blk_first);
-        else pack_multi_kernel<false><<<tp->pack_blocks, 256, 0, st>>>(tp->pack_dev, tp->pack_blk_job, tp->pack_blk_first);
+        pack_multi_kernel<true><<<tp->pack_blocks, 256, 0, st>>>(tp->pack_dev, tp->pack_blk_job, tp->pack_blk_first);
         ctx->launches++;
     }
     for (const PackFoldParams& fp : tp->pack_fold_jobs) {
         const size_t n = (size_t)fp.kh * fp.cout_pad * fp.kfold;
         const int blocks = (int)std::min<size_t>((n + 255) / 256, 4096);
-        if (ctx->bf16) pack_fold_kernel<true><<<blocks, 256, 0, st>>>(fp);
-        else pack_fold_kernel<false><<<blocks, 256, 0, st>>>(fp);
+        pack_fold_kernel<true><<<blocks, 256, 0, st>>>(fp);
         ctx->launches++;
     }
     for (const FoldJob& f : tp->fold_jobs) {
@@ -647,12 +678,10 @@ static int launch_ingest(w2l_ctx* ctx, const Op& op, const void* src, cudaStream
     const bool vec4 = ip.lo_off == 0 && ((ip.W | ip.Wsrc) & 3) == 0 && ((ip.sB | ip.sC | ip.sT | ip.sG) & 3) == 0 && (((uintptr_t)ip.src) & 15) == 0;
     if (vec4) {
         const int blocks = (int)std::min<long long>((total / 4 + 255) / 256, ctx->num_sms * 16);
-        if (ctx->bf16) ingest4_kernel<true><<<blocks, 256, 0, st>>>(ip);
-        else ingest4_kernel<false><<<blocks, 256, 0, st>>>(ip);
+        ingest4_kernel<true><<<blocks, 256, 0, st>>>(ip);
     } else {
         const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-        if (ctx->bf16) ingest_kernel<true><<<blocks, 256, 0, st>>>(ip);
-        else ingest_kernel<false><<<blocks, 256, 0, st>>>(ip);
+        ingest_kernel<true><<<blocks, 256, 0, st>>>(ip);
     }
     ctx->launches++;
     return W2L_OK;
@@ -665,8 +694,7 @@ constexpr int kRedSmem = 2 * 2048 * 4;   // chan_reduce_kernel: [rows][2][C] flo
 
 template <int MODE>
 static void launch_chan_reduce(w2l_ctx* ctx, const ChanReduceParams& rp, int nblk, cudaStream_t st) {
-    if (ctx->bf16) chan_reduce_kernel<true, MODE><<<nblk, kBnThreads, kRedSmem, st>>>(rp);
-    else chan_reduce_kernel<false, MODE><<<nblk, kBnThreads, kRedSmem, st>>>(rp);
+    chan_reduce_kernel<true, MODE><<<nblk, kBnThreads, kRedSmem, st>>>(rp);
     ctx->launches++;
 }
 
@@ -688,8 +716,7 @@ static int block_forward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool update_run
     ap.y = b.y.ptr(); ap.y_pitch = b.y.Cs; ap.y_f32 = b.y_f32;
     ap.stats = b.stats; ap.M = b.M; ap.C = C;
     const int grid = b.nblk * 2;   // rows-of-pixels layout (kBnThreads / (C/8) pixels per block iteration), as the reductions
-    if (ctx->bf16) bn_apply_kernel<true><<<grid, kBnThreads, 0, st>>>(ap);
-    else bn_apply_kernel<false><<<grid, kBnThreads, 0, st>>>(ap);
+    bn_apply_kernel<true><<<grid, kBnThreads, 0, st>>>(ap);
     ctx->launches++;
     return W2L_OK;
 }
@@ -741,8 +768,7 @@ static int block_backward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool wgrad, bo
         ap.dz = b.dz.ptr(); ap.du = b.L.residual ? b.du.ptr() : nullptr; ap.stats = b.stats; ap.coef = b.coef; ap.M = b.M; ap.C = C;
         if (mask_from_z) ap.y = nullptr;
         const int grid = b.nblk * 2;
-        if (ctx->bf16) bn_bwd_apply_kernel<true><<<grid, kBnThreads, 0, st>>>(ap);
-        else bn_bwd_apply_kernel<false><<<grid, kBnThreads, 0, st>>>(ap);
+        bn_bwd_apply_kernel<true><<<grid, kBnThreads, 0, st>>>(ap);
         ctx->launches++;
         // the conv bias under a BatchNorm has an exactly zero gradient (sum of dz over the batch is 0 by construction)
         if (wgrad && b.gb && !accumulate) { fill_kernel<<<1, 128, 0, st>>>(b.gb, C, 0.0f); ctx->launches++; }
@@ -803,8 +829,7 @@ static int train_forward(w2l_ctx* ctx, TrainPlan* tp, const void* in0, const voi
         hp.y32 = tp->y32.ptr(); hp.y_pitch = tp->y32.Cs; hp.w = hw; hp.b = hb; hp.g = (float*)out0;
         hp.N = tp->N; hp.B = tp->T > 0 ? tp->B : tp->N; hp.T = tp->T > 0 ? tp->T : 1; hp.HW = 9216;
         const int grid = elem_grid(ctx, (long long)tp->N * 9216);
-        if (ctx->bf16) head_fwd_kernel<true><<<grid, 256, 0, st>>>(hp);
-        else head_fwd_kernel<false><<<grid, 256, 0, st>>>(hp);
+        head_fwd_kernel<true><<<grid, 256, 0, st>>>(hp);
         ctx->launches++;
         tp->g_out = (const float*)out0;
     } else if (tp->net == W2L_NET_SYNCNET) {
@@ -816,8 +841,7 @@ static int train_forward(w2l_ctx* ctx, TrainPlan* tp, const void* in0, const voi
         float *hw, *hb;
         CKR(bound_ptr(ts, tp->net, "binary_pred.0.weight", 512, &hw, nullptr));
         CKR(bound_ptr(ts, tp->net, "binary_pred.0.bias", 1, &hb, nullptr));
-        if (ctx->bf16) disc_head_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->feat.ptr(), hw, hb, (float*)out0, tp->N, 512, tp->feat.Cs, 0);
-        else disc_head_kernel<false><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->feat.ptr(), hw, hb, (float*)out0, tp->N, 512, tp->feat.Cs, 0);
+        disc_head_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->feat.ptr(), hw, hb, (float*)out0, tp->N, 512, tp->feat.Cs, 0);
         ctx->launches++;
         tp->prob_out = (const float*)out0;
     }
@@ -841,20 +865,14 @@ static int train_backward(w2l_ctx* ctx, TrainPlan* tp, const float* d0, const fl
         hp.y32 = tp->y32.ptr(); hp.y_pitch = tp->y32.Cs; hp.w = hw; hp.b = hb; hp.g = const_cast<float*>(tp->g_out); hp.dg = d0;
         hp.dy32 = tp->dy32.ptr(); hp.partial = tp->head_partial;
         hp.N = tp->N; hp.B = tp->T > 0 ? tp->B : tp->N; hp.T = tp->T > 0 ? tp->T : 1; hp.HW = 9216;
-        if (ctx->bf16) head_bwd_kernel<true><<<tp->head_blocks, 256, 0, st>>>(hp);
-        else head_bwd_kernel<false><<<tp->head_blocks, 256, 0, st>>>(hp);
+        head_bwd_kernel<true><<<tp->head_blocks, 256, 0, st>>>(hp);
         ctx->launches++;
         if (wgrad && ghw && ghb) { head_bwd_finalize_kernel<<<1, 128, 0, st>>>(tp->head_partial, tp->head_blocks, ghw, ghb, acc ? 1 : 0); ctx->launches++; }
     } else if (tp->net == W2L_NET_SYNCNET) {
         if (!tp->a_out) return fail(W2L_ESTATE, "syncnet backward before a training forward");
         // through F.normalize (syncnet.py:62-63): d0 = dL/d audio_embedding, d1 = dL/d face_embedding
-        if (ctx->bf16) {
-            l2norm_bwd_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->ae_raw, d0, tp->dae.ptr(), tp->N, 512);
-            l2norm_bwd_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->fe_raw, d1, tp->dfe.ptr(), tp->N, 512);
-        } else {
-            l2norm_bwd_kernel<false><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->ae_raw, d0, tp->dae.ptr(), tp->N, 512);
-            l2norm_bwd_kernel<false><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->fe_raw, d1, tp->dfe.ptr(), tp->N, 512);
-        }
+        l2norm_bwd_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->ae_raw, d0, tp->dae.ptr(), tp->N, 512);
+        l2norm_bwd_kernel<true><<<(tp->N + 3) / 4, 128, 0, st>>>(tp->fe_raw, d1, tp->dfe.ptr(), tp->N, 512);
         ctx->launches += 2;
     } else {
         if (!tp->prob_out) return fail(W2L_ESTATE, "disc backward before a training forward");
@@ -864,8 +882,7 @@ static int train_backward(w2l_ctx* ctx, TrainPlan* tp, const float* d0, const fl
         float* dw = (wgrad && ghw) ? ghw : ts->loss_dev + 8;   // scratch when the head's gradient is not wanted
         float* db = (wgrad && ghb) ? ghb : ts->loss_dev + 8 + 512;
         const int accf = (wgrad && ghw && acc) ? 1 : 0;
-        if (ctx->bf16) disc_head_bwd_kernel<true><<<1, 512, 0, st>>>(tp->feat.ptr(), tp->feat.Cs, hw, tp->prob_out, d0, tp->N, 512, tp->dfeat.ptr(), dw, db, accf);
-        else disc_head_bwd_kernel<false><<<1, 512, 0, st>>>(tp->feat.ptr(), tp->feat.Cs, hw, tp->prob_out, d0, tp->N, 512, tp->dfeat.ptr(), dw, db, accf);
+        disc_head_bwd_kernel<true><<<1, 512, 0, st>>>(tp->feat.ptr(), tp->feat.Cs, hw, tp->prob_out, d0, tp->N, 512, tp->dfeat.ptr(), dw, db, accf);
         ctx->launches++;
     }
     cudaStream_t s_wg = nullptr;

@@ -760,8 +760,7 @@ int w2l_train_backward(w2l_ctx* ctx, int net, const float* d0, const float* d1, 
         if (net == W2L_NET_SYNCNET && tp->T == 0) {
             const long long total = (long long)tp->N * 15 * 48 * 96;
             const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-            if (ctx->bf16) export_grad_kernel<true><<<blocks, 256, 0, st>>>(tp->dface_in.ptr(), tp->dface_in.Cs, dinput, tp->N, 48, 96, 15);
-            else export_grad_kernel<false><<<blocks, 256, 0, st>>>(tp->dface_in.ptr(), tp->dface_in.Cs, dinput, tp->N, 48, 96, 15);
+            export_grad_kernel<true><<<blocks, 256, 0, st>>>(tp->dface_in.ptr(), tp->dface_in.Cs, dinput, tp->N, 48, 96, 15);
         } else {
             GenLossGradParams lp;
             memset(&lp, 0, sizeof(lp));
@@ -769,8 +768,7 @@ int w2l_train_backward(w2l_ctx* ctx, int net, const float* d0, const float* d1, 
             if (net == W2L_NET_SYNCNET) lp.dsync = tp->dface_in.ptr(); else lp.ddisc = tp->dframes_in.ptr();
             const long long total = (long long)tp->B * 3 * tp->T * 9216;
             const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-            if (ctx->bf16) gen_loss_grad_kernel<true><<<blocks, 256, 0, st>>>(lp);
-            else gen_loss_grad_kernel<false><<<blocks, 256, 0, st>>>(lp);
+            gen_loss_grad_kernel<true><<<blocks, 256, 0, st>>>(lp);
         }
         ctx->launches++;
         CK(cudaGetLastError());
@@ -851,8 +849,7 @@ int w2l_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels, const float* x
     lp.g = ts->g_buf; lp.gt = gt; lp.dg = ts->dg_buf; lp.l1_scale = (1.0f - syncnet_wt) / (float)numel; lp.B = B; lp.T = T;
     {
         const int blocks = (int)std::min<long long>((numel + 255) / 256, ctx->num_sms * 16);
-        if (ctx->bf16) gen_loss_grad_kernel<true><<<blocks, 256, 0, st>>>(lp);
-        else gen_loss_grad_kernel<false><<<blocks, 256, 0, st>>>(lp);
+        gen_loss_grad_kernel<true><<<blocks, 256, 0, st>>>(lp);
         ctx->launches++;
     }
     CKR(generator_backward_dp(ctx, gp, ts->dg_buf, st));
@@ -980,7 +977,7 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     const bool s_fold = ctx->use_fold;
     ctx->use_fold = false;
     Act xin, dxin, yv, dyv, none;
-    size_t ws_need = 0;
+    size_t ws_need[2] = {0, 0};
     int r = tp_act(&tp, &xin, N, H, W, round_up(L.cin, 16));
     if (r == W2L_OK) r = tp_act(&tp, &dxin, N, H, W, round_up(L.cin, 16));
     if (r == W2L_OK) r = tp_act(&tp, &yv, N, Ho, Wo, L.cout);
@@ -989,10 +986,10 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
         add_train_ingest(&tp, "ingest.x", 0, xin, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W);
         add_train_ingest(&tp, "ingest.dy", 1, dyv, N, L.cout, (long long)L.cout * Ho * Wo, (long long)Ho * Wo, 0, 0, Wo);
         r = add_train_block(ctx, &tp, slot, 0, L, xin, yv, dyv, dx ? dxin : none, none, dw != nullptr,
-                            L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, &ws_need);
+                            L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, ws_need);
     }
     ctx->use_fold = s_fold;
-    if (r == W2L_OK && ws_need) { void* p = nullptr; r = plan_alloc(&tp.pl, &p, ws_need); tp.wg_ws = (float*)p; }
+    if (r == W2L_OK && ws_need[0]) { void* p = nullptr; r = plan_alloc(&tp.pl, &p, ws_need[0]); tp.wg_ws[0] = (float*)p; }
     if (r == W2L_OK) {
         cudaError_t e = cudaDeviceSynchronize();
         if (e != cudaSuccess) r = fail(W2L_ECUDA, "plan build failed: %s", cudaGetErrorString(e));
@@ -1003,8 +1000,7 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     if (r == W2L_OK) {
         const long long total = (long long)N * L.cout * Ho * Wo;
         const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-        if (ctx->bf16) export_kernel<true><<<blocks, 256, 0, st>>>(yv.base, y, N, Ho, Wo, L.cout, yv.Cs, 0, 0);
-        else export_kernel<false><<<blocks, 256, 0, st>>>(yv.base, y, N, Ho, Wo, L.cout, yv.Cs, 0, 0);
+        export_kernel<true><<<blocks, 256, 0, st>>>(yv.base, y, N, Ho, Wo, L.cout, yv.Cs, 0, 0);
         ctx->launches++;
     }
     if (r == W2L_OK && dy) {
@@ -1013,16 +1009,79 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
         if (r == W2L_OK && dx) {
             const long long total = (long long)N * L.cin * H * W;
             const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-            if (ctx->bf16) export_grad_kernel<true><<<blocks, 256, 0, st>>>(dxin.ptr(), dxin.Cs, dx, N, H, W, L.cin);
-            else export_grad_kernel<false><<<blocks, 256, 0, st>>>(dxin.ptr(), dxin.Cs, dx, N, H, W, L.cin);
+            export_grad_kernel<true><<<blocks, 256, 0, st>>>(dxin.ptr(), dxin.Cs, dx, N, H, W, L.cin);
             ctx->launches++;
         }
     }
     cudaError_t e = cudaStreamSynchronize(st);
     if (r == W2L_OK && e != cudaSuccess) r = fail(W2L_ECUDA, "conv block train failed: %s", cudaGetErrorString(e));
+    ts->last_block_info.clear();
+    if (r == W2L_OK) { ts->last_block_info.emplace_back(); train_block_info(ctx, &tp, tp.blocks[0], &ts->last_block_info.back()); }
     free_train_plan(&tp);
     ts->bound[slot].swap(saved);
     return r;
+}
+
+int w2l_debug_train_blocks(w2l_ctx* ctx, int net, int cap, w2l_train_block_info* out) {
+    if (!ctx || net < -1 || net > 2) return fail(W2L_EINVAL, "bad argument");
+    TrainState* ts = train_state(ctx);
+    std::vector<w2l_train_block_info> t;
+    if (net < 0) {
+        t = ts->last_block_info;
+    } else {
+        const TrainPlan* tp = ts->last[net];
+        if (!tp) return fail(W2L_ESTATE, "no training forward has run for net %d", net);
+        t.resize(tp->blocks.size());
+        for (size_t i = 0; i < tp->blocks.size(); ++i) train_block_info(ctx, tp, tp->blocks[i], &t[i]);
+    }
+    if (!out) return (int)t.size();
+    const int k = std::min<int>(std::max(cap, 0), (int)t.size());
+    for (int i = 0; i < k; ++i) out[i] = t[i];
+    return k;
+}
+
+int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* out, int* n, int* c, int* h, int* w, void* stream) {
+    if (!ctx || net < 0 || net > 2) return fail(W2L_EINVAL, "bad argument");
+    const TrainPlan* tp = train_state(ctx)->last[net];
+    if (!tp) return fail(W2L_ESTATE, "no training forward has run for net %d", net);
+    if (block < 0 || block >= (int)tp->blocks.size()) return fail(W2L_EINVAL, "block %d out of range", block);
+    const TBlock& b = tp->blocks[block];
+    const Act* a = nullptr;
+    int C = b.L.cout;
+    switch (which) {
+        case W2L_TAPE_X: a = &b.x; C = b.L.cin; break;
+        case W2L_TAPE_Z: a = &b.z; break;
+        case W2L_TAPE_Y: a = &b.y; break;
+        case W2L_TAPE_DY: a = &b.dy; break;
+        case W2L_TAPE_DZ: a = &b.dz; break;
+        case W2L_TAPE_DU: a = &b.du; break;
+        case W2L_TAPE_DX: a = &b.dx; C = b.L.cin; break;
+        case W2L_TAPE_DX_ADD: a = &b.dx_add; C = b.L.cin; break;
+        case W2L_TAPE_STATS: break;
+        default: return fail(W2L_EINVAL, "unknown tape tensor %d", which);
+    }
+    if (which == W2L_TAPE_STATS) {
+        if (!b.bn) return fail(W2L_EINVAL, "%s has no BatchNorm statistics", b.L.name.c_str());
+        if (n) *n = 2;
+        if (c) *c = C;
+        if (h) *h = 1;
+        if (w) *w = 1;
+        if (out) CK(cudaMemcpyAsync(out, b.stats, (size_t)2 * C * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+        return W2L_OK;
+    }
+    if (!a->base) return fail(W2L_EINVAL, "%s has no tape tensor %d", b.L.name.c_str(), which);
+    if (n) *n = a->N;
+    if (c) *c = C;
+    if (h) *h = a->H;
+    if (w) *w = a->W;
+    if (!out) return W2L_OK;
+    DeviceGuard g(ctx->device);
+    const long long total = (long long)a->N * C * a->H * a->W;
+    const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
+    export_grad_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(a->ptr(), a->Cs, out, a->N, a->H, a->W, C);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return W2L_OK;
 }
 
 int64_t w2l_launch_count(const w2l_ctx* ctx) { return ctx ? ctx->launches : 0; }
