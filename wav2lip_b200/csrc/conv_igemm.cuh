@@ -16,18 +16,23 @@
 //             coordinates are zero-filled by the TMA unit, which IS the conv zero padding) and one
 //             3-D TMA load brings the [BN x BK] weight slice of that tap. Both land K-major with the
 //             hardware 128/64/32-byte swizzle that the wgmma shared-memory descriptors expect.
-//   warps 4+: one consumer warpgroup per M tile (MT = 2: two tiles that share every weight slab, half the
-//             weight traffic per FLOP).  It issues wgmma.mma_async m64nBNk16 for both 64-row halves of its tile,
+//   warps 4-11: two consumer warpgroups.  MT = 2: one per M tile of a unit (two tiles that share every weight
+//             slab, half the weight traffic per FLOP).  MT = 1 (ping-pong): they take alternate tiles of the CTA and
+//             their K loops alternate (a pair of named barriers hands the ring over), so one warpgroup's epilogue
+//             runs while the other issues MMAs.  The producer warpgroup gives registers to the consumers
+//             (setmaxnreg).  A warpgroup issues wgmma.mma_async m64nBNk16 for both 64-row halves of its tile,
 //             accumulating in registers (fp32), keeps one K step in flight and releases each shared-memory
-//             stage as soon as the step that read it has retired.  Then the epilogue: the accumulator goes
-//             through a small shared-memory transpose (wgmma.cuh: acc_to_rows) so that thread = GEMM row =
-//             output pixel, the folded BatchNorm scale/shift (conv bias folded in), the residual add
-//             (conv.py:16-18: after BN, before ReLU), ReLU / LeakyReLU(0.01), and NHWC 16-bit straight into the
-//             channel slice of the consumer's buffer (so torch.cat of wav2lip.py:108 never exists).
-//             Staged mode (tma_epi): the residual tile arrives by TMA into a swizzled shared-memory tile,
-//             is combined in place and leaves by ONE TMA tensor store per 64 channels (which also clips
-//             ragged tiles); direct mode (fp32 outputs, fused generator head wav2lip.py:84-85): per-thread
-//             global accesses.  While a warpgroup runs its epilogue the producer keeps filling the ring.
+//             stage as soon as the step that read it has retired.  Then the epilogue: the folded BatchNorm
+//             scale/shift (conv bias folded in), the residual add (conv.py:16-18: after BN, before ReLU), ReLU /
+//             LeakyReLU(0.01), and NHWC 16-bit straight into the channel slice of the consumer's buffer (so
+//             torch.cat of wav2lip.py:108 never exists).
+//             Staged mode (tma_epi): works on the wgmma accumulator fragment itself.  The residual arrives by TMA
+//             in the warpgroup's swizzled staging boxes (the full tile width, one box per 64 channels), every
+//             column pair is combined in place at its swizzled address, and the boxes leave by TMA tensor stores
+//             (which also clip ragged tiles); the next tile's residual is requested as soon as the stores have
+//             read the boxes.  Direct mode (fp32 outputs, split-operand mode, fused generator head
+//             wav2lip.py:84-85): a shared-memory transpose (wgmma.cuh: acc_to_rows) makes thread = GEMM row =
+//             output pixel, then per-thread global accesses.
 //
 // Everything a launch needs is in ConvParams (a __grid_constant__), built once per plan on the host.
 #pragma once
@@ -167,24 +172,32 @@ __device__ __forceinline__ void wg_mma_tile(float (&acc)[2][BN / 2], uint32_t a,
     }
 }
 
-// MT = number of 128-row M tiles a CTA works on at once (sharing each weight slab), one consumer warpgroup each.
+// MT = number of 128-row M tiles a CTA works on at once (sharing each weight slab).  Either way the CTA has two
+// consumer warpgroups: MT = 2 gives each one of the unit's two tiles, MT = 1 gives them alternate tiles (ping-pong).
+// Shared memory: the K-step ring, then one region per consumer warpgroup that holds either the staging boxes of the
+// staged epilogue (the full tile width, BN / kEW boxes) or the transpose buffer of the direct one (a launch uses one
+// epilogue form), then the barriers.
 template <int BN, int BK, int MT = 1>
 struct ConvCfg {
     static constexpr int kATile = kTileM * BK * 2;
     static constexpr int kABytes = MT * kATile;
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kEW = BN < 64 ? BN : 64;                 // channels per epilogue pass
-    static constexpr int kCW = BN < 32 ? BN : 32;                 // accumulator columns per transpose chunk
-    static constexpr int kStgTile = kTileM * kEW * 2;             // staging tile of one epilogue group
-    static constexpr int kStgBytes = MT * ((kStgTile + 1023) / 1024 * 1024);
-    static constexpr int kXBytes = MT * xbuf_bytes<kCW>();
-    static constexpr int kStagesRaw = (kSmemMax - kSmemExtra - kStgBytes - kXBytes) / kStageBytes;
+    static constexpr int kEW = BN < 64 ? BN : 64;                 // channels per epilogue box (one TMA box)
+    static constexpr int kCW = BN < 32 ? BN : 32;                 // accumulator columns per transpose chunk (direct epilogue)
+    static constexpr int kPasses = BN / kEW;                      // epilogue boxes per tile
+    static constexpr int kBoxBytes = kTileM * kEW * 2;            // one staging box: 128 rows x kEW 16-bit channels
+    static constexpr int kGrpRaw = kPasses * kBoxBytes > xbuf_bytes<kCW>() ? kPasses * kBoxBytes : xbuf_bytes<kCW>();
+    static constexpr int kGrpBytes = (kGrpRaw + 1023) / 1024 * 1024;  // epilogue region of one consumer warpgroup
+    static constexpr int kStagesRaw = (kSmemMax - kSmemExtra - 2 * kGrpBytes) / kStageBytes;
     static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-    static constexpr int kSmemBytes = kStages * kStageBytes + kStgBytes + kXBytes + kSmemExtra;
-    static constexpr int kThreads = 128 + 128 * MT;  // the producer warpgroup + one consumer warpgroup per M tile
+    static constexpr int kRingBytes = (kStages * kStageBytes + 1023) / 1024 * 1024;
+    static constexpr int kSmemBytes = kRingBytes + 2 * kGrpBytes + kSmemExtra;
+    static constexpr int kThreads = 384;  // the producer warpgroup + two consumer warpgroups
     static_assert(BN <= 128, "a warpgroup holds at most 128 fp32 accumulator columns per row");
+    static_assert(kBoxBytes % 1024 == 0, "staging boxes must keep the 1024-byte swizzle alignment");
     static_assert(kStages >= 2, "need a pipeline");
+    static_assert(kSmemBytes <= kSmemMax, "shared-memory carve-up exceeds the per-CTA limit");
 };
 
 // Sticky range flag of the fp16 modes: set by any epilogue that rounds a value beyond the fp16 range (|v| > 65504 ->
@@ -316,19 +329,30 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
+// Register split between the warpgroups (all four warps of a warpgroup execute it): the producer needs few registers, the
+// consumers hold a 128 x BN fp32 accumulator tile each.  __launch_bounds__(384, 1) gives every thread 168; 128 x 40 +
+// 256 x 232 = 64 512 of the SM's 65 536.
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
 template <int BN, int BK, bool kBF16, bool kHead, int MT = 1>
 __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
     pdl_launch_dependents();
     using Cfg = ConvCfg<BN, BK, MT>;
     constexpr int kStages = Cfg::kStages;
     static_assert(!kHead || BN == 32, "fused head expects the 32-channel output block");
+    static_assert(MT == 1 || MT == 2, "one or two M tiles per unit");
 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_raw_u32 = smem_u32(smem_raw);
     const uint32_t smem_base = (smem_raw_u32 + 1023u) & ~1023u;  // swizzle atoms need 1024-B alignment
-    const uint32_t stg_base = smem_base + kStages * Cfg::kStageBytes;
-    const uint32_t xb_base = stg_base + Cfg::kStgBytes;
-    const uint32_t bar_base = xb_base + Cfg::kXBytes;
+    const uint32_t grp_base = smem_base + Cfg::kRingBytes;       // the two consumer warpgroups' epilogue regions
+    const uint32_t bar_base = grp_base + 2 * Cfg::kGrpBytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
     auto res_bar = [&](int g) { return bar_base + 8u * (2 * kStages + g); };
@@ -347,9 +371,9 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 4 * MT);  // one arrive per consumer warp
+            mbar_init(empty_bar(s), 4 * MT);  // one arrive per warp of the warpgroup(s) that consume the step
         }
-        for (int g = 0; g < MT; ++g) mbar_init(res_bar(g), 1);
+        for (int g = 0; g < 2; ++g) mbar_init(res_bar(g), 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -360,9 +384,10 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
     const int total_tiles = m_units * p.n_tiles;  // end decodes to n >= N: its loads are zero-filled, its rows masked)
     const int k_steps = p.ntaps * p.kc_per_tap;
 
-    if (warp == 0) {
-        // =============================== TMA producer ===============================
-        if (lane == 0) {
+    if (warp < 4) {
+        setmaxnreg_dec<kProducerRegs>();
+        // =============================== TMA producer: K steps in tile order into the one ring ===============================
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -395,22 +420,31 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
                 }
             }
         }
-    } else if (warp >= 4) {
+    } else {
+        setmaxnreg_inc<kConsumerRegs>();
         // =============================== consumer warpgroups: MMA + epilogue ===============================
+        // MT = 2: group g computes M tile g of every unit of the CTA.  MT = 1 (ping-pong): group g takes the CTA's tiles
+        // i = g, g + 2, ..., so one group's epilogue runs while the other issues MMAs.  Tile i of the CTA is
+        // blockIdx.x + i * gridDim.x; its K steps are the CTA-global ring steps i * k_steps + ks.
+        const int g = (warp - 4) >> 2;     // consumer warpgroup
         const int q = (warp - 4) & 3;      // warp of the warpgroup
-        const int mt = (warp - 4) >> 2;    // which of the unit's M tiles this warpgroup computes
-        const int row = q * 32 + lane;     // GEMM row == pixel index inside the tile box (after the transpose)
+        const int mt = MT == 2 ? g : 0;    // which of the unit's M tiles this warpgroup computes
+        constexpr int kItStride = MT == 2 ? 1 : 2;
+        const int it0 = MT == 2 ? 0 : g;
         const int rows_valid = p.bw * p.bh * p.bn;
-        const int px = row % p.bw;
-        const int py = (row / p.bw) % p.bh;
-        const int pn = row / (p.bw * p.bh);
-        const uint32_t bar_id = 1 + mt;    // named barrier of this warpgroup (0 is __syncthreads)
-        float* const xb = reinterpret_cast<float*>(smem_raw + (xb_base - smem_raw_u32) + mt * xbuf_bytes<Cfg::kCW>());
+        const uint32_t bar_id = 1 + g;     // named barrier of this warpgroup (0 is __syncthreads)
+        // MT = 1: the two groups' K loops alternate.  Group g waits on named barrier 3 + g before its K loop; the other
+        // group arrives there once it has waited for the last full barrier of its own tile.  So every ring step before
+        // a group's first one has been loaded when the group starts, and a parity wait can never see a stage two
+        // phases behind.
+        const uint32_t my_turn = 3 + g, their_turn = 3 + (g ^ 1);
+        const uint32_t grp = grp_base + g * Cfg::kGrpBytes;
         float acc[2][BN / 2];
-        int stage = 0;
-        uint32_t phase = 0;
-        // the K loop of one unit; one wgmma group stays in flight, the stage of the step before it is released
-        auto mainloop = [&]() {
+        // the K loop of one tile (ring steps s0 ..); one wgmma group stays in flight, the stage of the step before it is
+        // released; hand_off = the other group has a next tile and waits for this K loop
+        auto mainloop = [&](int s0, bool hand_off) {
+            int stage = s0 % kStages;
+            uint32_t phase = static_cast<uint32_t>(s0 / kStages) & 1u;
             int prev = -1;
             for (int ks = 0; ks < k_steps; ++ks) {
                 mbar_wait(full_bar(stage), phase);
@@ -423,132 +457,135 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
                 prev = stage;
                 if (++stage == kStages) { stage = 0; phase ^= 1u; }
             }
+            if (hand_off) named_bar_arrive(their_turn, 256);
             wg_wait<0>();
             wg_fence_regs<BN / 2>(acc[0]);
             wg_fence_regs<BN / 2>(acc[1]);
             if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         };
+        // every tile of this warpgroup: K loop, then epilogue(tile, next tile of this group exists)
+        auto for_each_tile = [&](auto&& epilogue) {
+            for (int it = it0;; it += kItStride) {
+                const int tile = blockIdx.x + it * static_cast<int>(gridDim.x);
+                if (tile >= total_tiles) break;
+                if (MT == 1 && it > 0) named_bar_sync(my_turn, 256);
+                mainloop(it * k_steps, MT == 1 && tile + static_cast<int>(gridDim.x) < total_tiles);
+                epilogue(tile, tile + kItStride * static_cast<int>(gridDim.x) < total_tiles);
+            }
+        };
+        auto tile_origin = [&](int tile_, int* nt_, int* x0_, int* y0_, int* n0_) {
+            *nt_ = tile_ % p.n_tiles;
+            const int m_ = (tile_ / p.n_tiles) * MT + mt;
+            *x0_ = (m_ % p.tiles_x) * p.bw;
+            *y0_ = ((m_ / p.tiles_x) % p.tiles_y) * p.bh;
+            *n0_ = (m_ / (p.tiles_x * p.tiles_y)) * p.bn;
+        };
         if (!kHead && p.tma_epi) {
-            // ---- staged epilogue: residual in by TMA, result out by TMA, one swizzled smem tile per group ----
+            // ---- staged epilogue on the accumulator fragment: the residual arrives by TMA in the warpgroup's swizzled
+            // staging boxes (one per kEW channels), every value is combined in place and the boxes leave by TMA stores ----
             constexpr int EW = Cfg::kEW;
-            constexpr int CW = Cfg::kCW;
-            constexpr int kPasses = BN / EW;
+            constexpr int kPasses = Cfg::kPasses;
             constexpr uint32_t kRowB = EW * 2;
             constexpr uint32_t kSwz = (kRowB == 128) ? 7u : (kRowB == 64) ? 3u : 1u;
-            const uint32_t stg = stg_base + mt * ((Cfg::kStgTile + 1023) / 1024 * 1024);
             const bool leader = (q == 0 && lane == 0);
             const bool has_res = p.ep.res != nullptr;
             const EpiParams& e = p.ep;
-            auto tile_origin = [&](int tile_, int* nt_, int* x0_, int* y0_, int* n0_) {
-                *nt_ = tile_ % p.n_tiles;
-                const int m_ = (tile_ / p.n_tiles) * MT + mt;
-                *x0_ = (m_ % p.tiles_x) * p.bw;
-                *y0_ = ((m_ / p.tiles_x) % p.tiles_y) * p.bh;
-                *n0_ = (m_ / (p.tiles_x * p.tiles_y)) * p.bn;
+            // leader: request all residual boxes of a tile (the staging boxes must be free)
+            auto fetch_res = [&](int tile_) {
+                int nt_, x0_, y0_, n0_;
+                tile_origin(tile_, &nt_, &x0_, &y0_, &n0_);
+                mbar_arrive_expect_tx(res_bar(g), kPasses * p.epi_box_bytes);
+#pragma unroll
+                for (int ps = 0; ps < kPasses; ++ps)
+                    tma_load_4d(grp + ps * Cfg::kBoxBytes, &p.tmR, res_bar(g), nt_ * BN + ps * EW, x0_, y0_, n0_);
             };
-            uint32_t rphase = 0;
-            if (has_res && leader && static_cast<int>(blockIdx.x) < total_tiles) {
-                int nt0, x0, y0, n0;
-                tile_origin(blockIdx.x, &nt0, &x0, &y0, &n0);
-                mbar_arrive_expect_tx(res_bar(mt), p.epi_box_bytes);
-                tma_load_4d(stg, &p.tmR, res_bar(mt), nt0 * BN, x0, y0, n0);
+            if (has_res && leader) {
+                const int first = blockIdx.x + it0 * static_cast<int>(gridDim.x);
+                if (first < total_tiles) fetch_res(first);
             }
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            uint32_t rphase = 0;
+            for_each_tile([&](int tile, bool more) {
                 int nt, x0, y0, n0;
                 tile_origin(tile, &nt, &x0, &y0, &n0);
-                mainloop();
-#pragma unroll
-                for (int ps = 0; ps < kPasses; ++ps) {
-                    if (has_res) {
-                        mbar_wait(res_bar(mt), rphase);
-                        rphase ^= 1u;
-                    }
-                    const int cg = nt * BN + ps * EW;
-#pragma unroll
-                    for (int c0 = 0; c0 < EW; c0 += CW) {
-                    uint32_t v[CW];
-                    acc_to_rows<CW>(acc[0], acc[1], ps * EW + c0, xb, bar_id, v);
-#pragma unroll
-                    for (int jj = 0; jj < CW / 8; ++jj) {
-                        const int j = c0 / 8 + jj;
-                        float f[8];
-                        const float4 s0 = __ldg(reinterpret_cast<const float4*>(e.scale + cg + 8 * j));
-                        const float4 s1 = __ldg(reinterpret_cast<const float4*>(e.scale + cg + 8 * j + 4));
-                        const float4 h0 = __ldg(reinterpret_cast<const float4*>(e.shift + cg + 8 * j));
-                        const float4 h1 = __ldg(reinterpret_cast<const float4*>(e.shift + cg + 8 * j + 4));
-                        f[0] = fmaf(__uint_as_float(v[8 * jj + 0]), s0.x, h0.x);
-                        f[1] = fmaf(__uint_as_float(v[8 * jj + 1]), s0.y, h0.y);
-                        f[2] = fmaf(__uint_as_float(v[8 * jj + 2]), s0.z, h0.z);
-                        f[3] = fmaf(__uint_as_float(v[8 * jj + 3]), s0.w, h0.w);
-                        f[4] = fmaf(__uint_as_float(v[8 * jj + 4]), s1.x, h1.x);
-                        f[5] = fmaf(__uint_as_float(v[8 * jj + 5]), s1.y, h1.y);
-                        f[6] = fmaf(__uint_as_float(v[8 * jj + 6]), s1.z, h1.z);
-                        f[7] = fmaf(__uint_as_float(v[8 * jj + 7]), s1.w, h1.w);
-                        uint32_t a = stg + row * kRowB + j * 16;
-                        a ^= ((a >> 7) & kSwz) << 4;
-                        if (has_res) {
-                            uint32_t r0, r1, r2, r3;
-                            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(a));
-                            const float2 a0 = unpack2<kBF16>(r0), a1 = unpack2<kBF16>(r1);
-                            const float2 a2 = unpack2<kBF16>(r2), a3 = unpack2<kBF16>(r3);
-                            f[0] += a0.x; f[1] += a0.y; f[2] += a1.x; f[3] += a1.y;
-                            f[4] += a2.x; f[5] += a2.y; f[6] += a3.x; f[7] += a3.y;
-                        }
-                        if (e.act == ACT_RELU) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) f[i] = fmaxf(f[i], 0.0f);
-                        } else if (e.act == ACT_LRELU) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) f[i] = f[i] > 0.0f ? f[i] : 0.01f * f[i];
-                        }
-                        const bool live = row < rows_valid;
-                        const uint32_t o0 = pack2<kBF16>(f[0], f[1], live), o1 = pack2<kBF16>(f[2], f[3], live);
-                        const uint32_t o2 = pack2<kBF16>(f[4], f[5], live), o3 = pack2<kBF16>(f[6], f[7], live);
-                        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a), "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
-                    }
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-                    if (leader) {
-                        asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                                     ::"l"(reinterpret_cast<uint64_t>(&p.tmO)), "r"(stg), "r"(cg), "r"(x0), "r"(y0), "r"(n0)
-                                     : "memory");
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the store has read the tile
-                        if (has_res) {  // fetch the residual of the next pass / next tile into the (now free) tile
-                            int nnt = nt, nx0 = x0, ny0 = y0, nn0 = n0, nps = ps + 1;
-                            bool more = true;
-                            if (nps == kPasses) {
-                                nps = 0;
-                                const int ntile = tile + static_cast<int>(gridDim.x);
-                                more = ntile < total_tiles;
-                                if (more) tile_origin(ntile, &nnt, &nx0, &ny0, &nn0);
-                            }
-                            if (more) {
-                                mbar_arrive_expect_tx(res_bar(mt), p.epi_box_bytes);
-                                tma_load_4d(stg, &p.tmR, res_bar(mt), nnt * BN + nps * EW, nx0, ny0, nn0);
-                            }
-                        }
-                    }
-                    // everyone else must not touch the tile again before the leader is past wait_group.read
-                    asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+                if (has_res) {
+                    mbar_wait(res_bar(g), rphase);
+                    rphase ^= 1u;
                 }
-            }
+                // fragment of m64nBNk16: this thread holds rows 16q + lane/4 (+8) of each 64-row half and, in every
+                // 8-column chunk j, the column pair 8j + 2(lane%4)
+                const float* const scale = e.scale + nt * BN;
+                const float* const shift = e.shift + nt * BN;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    const float2 sc = __ldg(reinterpret_cast<const float2*>(scale + c));
+                    const float2 sh = __ldg(reinterpret_cast<const float2*>(shift + c));
+                    const uint32_t box = grp + (8 * j / EW) * Cfg::kBoxBytes;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                        for (int r8 = 0; r8 < 2; ++r8) {
+                            const int row = 64 * h + 16 * q + (lane >> 2) + 8 * r8;
+                            float f0 = fmaf(acc[h][4 * j + 2 * r8], sc.x, sh.x);
+                            float f1 = fmaf(acc[h][4 * j + 2 * r8 + 1], sc.y, sh.y);
+                            uint32_t a = box + row * kRowB + (c % EW) * 2;
+                            a ^= ((a >> 7) & kSwz) << 4;
+                            if (has_res) {
+                                uint32_t r;
+                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(a));
+                                const float2 rv = unpack2<kBF16>(r);
+                                f0 += rv.x;
+                                f1 += rv.y;
+                            }
+                            if (e.act == ACT_RELU) {
+                                f0 = fmaxf(f0, 0.0f);
+                                f1 = fmaxf(f1, 0.0f);
+                            } else if (e.act == ACT_LRELU) {
+                                f0 = f0 > 0.0f ? f0 : 0.01f * f0;
+                                f1 = f1 > 0.0f ? f1 : 0.01f * f1;
+                            }
+                            const uint32_t o = pack2<kBF16>(f0, f1, row < rows_valid);
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(o) : "memory");
+                        }
+                    }
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
+                named_bar_sync(bar_id, 128);
+                if (leader) {
+#pragma unroll
+                    for (int ps = 0; ps < kPasses; ++ps)
+                        asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                                     ::"l"(reinterpret_cast<uint64_t>(&p.tmO)), "r"(grp + ps * Cfg::kBoxBytes), "r"(nt * BN + ps * EW),
+                                       "r"(x0), "r"(y0), "r"(n0)
+                                     : "memory");
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the stores have read the boxes
+                    // the next tile's residual lands while the other warpgroup runs its MMAs
+                    if (has_res && more) fetch_res(tile + kItStride * static_cast<int>(gridDim.x));
+                }
+                // nobody writes the boxes again before the stores have read them: with a residual the next epilogue
+                // waits for its TMA load (issued after the read), without one the whole group waits here
+                if (has_res)
+                    __syncwarp();
+                else
+                    named_bar_sync(bar_id, 128);
+            });
             if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
         } else {
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int nt = tile % p.n_tiles;
-                const int m = (tile / p.n_tiles) * MT + mt;
-                const int tx = m % p.tiles_x;
-                const int ty = (m / p.tiles_x) % p.tiles_y;
-                const int tn = m / (p.tiles_x * p.tiles_y);
-                const int x = tx * p.bw + px;
-                const int y = ty * p.bh + py;
-                const int n = tn * p.bn + pn;
+            // ---- direct epilogue (fused head, fp32 outputs, split-operand mode): transpose through the warpgroup's
+            // region so that thread = GEMM row = output pixel, then per-thread global accesses ----
+            const int row = q * 32 + lane;
+            const int px = row % p.bw;
+            const int py = (row / p.bw) % p.bh;
+            const int pn = row / (p.bw * p.bh);
+            float* const xb = reinterpret_cast<float*>(smem_raw + (grp - smem_raw_u32));
+            for_each_tile([&](int tile, bool) {
+                int nt, x0, y0, n0;
+                tile_origin(tile, &nt, &x0, &y0, &n0);
+                const int x = x0 + px, y = y0 + py, n = n0 + pn;
                 const bool valid = (row < rows_valid) && (x < p.ep.Wout) && (y < p.ep.Hout) && (n < p.ep.N);
-                mainloop();
                 epilogue_tile<BN, kBF16, kHead>(p.ep, acc, xb, bar_id, valid, n, y, x, nt);
-            }
+            });
         }
     }
 }

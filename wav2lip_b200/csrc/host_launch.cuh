@@ -9,12 +9,12 @@
 typedef void (*ConvKernelFn)(const ConvParams);
 struct ConvKernelEntry { int BN, BK; bool bf16, head; ConvKernelFn fn; int smem; uint64_t attr_set; int mt; int threads; };
 
-#define W2L_CONV_ENTRY(BN_, BK_)                                                                                               \
-    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, 256},         \
-    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, 256}
-#define W2L_CONV_ENTRY_MT2(BN_, BK_)                                                                                           \
-    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, 384},   \
-    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, 384}
+#define W2L_CONV_ENTRY(BN_, BK_)                                                                                                        \
+    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads}, \
+    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads}
+#define W2L_CONV_ENTRY_MT2(BN_, BK_)                                                                                                    \
+    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads}, \
+    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads}
 
 static ConvKernelEntry g_conv_kernels[] = {
     W2L_CONV_ENTRY(16, 16), W2L_CONV_ENTRY(16, 32), W2L_CONV_ENTRY(16, 64),
@@ -22,8 +22,8 @@ static ConvKernelEntry g_conv_kernels[] = {
     W2L_CONV_ENTRY(64, 16), W2L_CONV_ENTRY(64, 32), W2L_CONV_ENTRY(64, 64),
     W2L_CONV_ENTRY(128, 16), W2L_CONV_ENTRY(128, 32), W2L_CONV_ENTRY(128, 64),
     W2L_CONV_ENTRY_MT2(64, 64), W2L_CONV_ENTRY_MT2(64, 32),
-    {32, 16, false, true, conv_igemm_kernel<32, 16, false, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, 256},
-    {32, 16, true, true, conv_igemm_kernel<32, 16, true, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, 256},
+    {32, 16, false, true, conv_igemm_kernel<32, 16, false, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads},
+    {32, 16, true, true, conv_igemm_kernel<32, 16, true, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads},
 };
 
 static ConvKernelEntry* find_conv_kernel(int BN, int BK, bool bf16, bool head, int mt = 1) {
