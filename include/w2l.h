@@ -145,11 +145,23 @@ int w2l_lipsync_frames_u8(w2l_ctx* ctx, const float* mel_dev, const uint8_t* fra
  * 3 L2Norm layers and the 12 mbox heads, max-out of the first scale's background logits included.
  *   img (B,3,H,W) fp32, BGR minus (104,117,123) as detect.py:21-23 / :60-61 prepare it  ->  12 maps
  *   outs[2i] = cls_i (B,2,h_i,w_i), outs[2i+1] = reg_i (B,4,h_i,w_i), i = 0..5 (strides 4..128), raw logits as the module
- *   returns them (softmax / threshold / decode / NMS of detect.py:31-56 and bbox.py:44-64 stay on the host side).
+ *   returns them (softmax / threshold / decode / NMS of detect.py:31-56 and bbox.py:44-64: w2l_s3fd_detect_u8 below).
  * w2l_s3fd_out_dims writes the six (h_i, w_i) pairs for an H x W input.  Weights: w2l_load_weights(ctx, W2L_NET_S3FD, ...)
  * with the module's own state_dict names ("conv1_1.weight", ..., "conv3_3_norm.weight", "conv7_2_mbox_loc.bias"). */
 int w2l_s3fd_out_dims(int H, int W, int32_t* dims12);
 int w2l_s3fd_forward(w2l_ctx* ctx, const float* img_dev, float* const* outs12_dev, int B, int H, int W, void* stream);
+
+/* The whole detector on the device: face_detection/detection/sfd detect.py:58-94 + bbox.py:44-64 + sfd_detector.py:40-46.
+ *   frames (B,H,W,3) uint8 in the order detect_from_batch takes them (reverse_channels = 1: reversed first, as api.py:64
+ *   does to the frames inference.py passes) -> per image the boxes that
+ *   survive greedy NMS at IoU 0.3 with score > 0.5, best first, at most max_det (>= 1) of them:
+ *   dets (B, max_det, 5) fp32 = x1 y1 x2 y2 score (rows past counts[b] are zero), counts (B) int32.
+ *   outs12: NULL, or the 12 maps of w2l_s3fd_forward, bit-identical to that call on the same frames.
+ * Only locations whose own score exceeds 0.5 can reach the output, so the reference's 0.05 threshold, its cross-image
+ * candidate union and their duplicates are not materialised; ties in score are ordered by descending location index
+ * (DESIGN.md §3.6).  Shares the S3FD plan of (B,H,W) with w2l_s3fd_forward. */
+int w2l_s3fd_detect_u8(w2l_ctx* ctx, const uint8_t* frames_dev, int B, int H, int W, int reverse_channels, int max_det,
+                       float* dets_dev, int32_t* counts_dev, float* const* outs12_dev, void* stream);
 
 /* Replaces `SyncNet_color.forward(audio, face)` (syncnet.py:55-66):
  *   mel (B,1,80,16), face (B,15,48,96) -> audio_emb (B,512), face_emb (B,512), both L2-normalised. */
@@ -233,6 +245,10 @@ int w2l_debug_kernel_table(int cap, w2l_kernel_info* out);
 /* the conv launches of the last plan of `net`; net = -1: of the last w2l_conv_block_forward call */
 int w2l_debug_plan_kernels(w2l_ctx* ctx, int net, int cap, w2l_kernel_info* out);
 /* Both return the number of entries written (at most cap), or a negative W2L_E* code; out == NULL returns the count. */
+/* The sorted pre-NMS candidates (score > 0.5) of `image` of the last S3FD call, which must have been w2l_s3fd_detect_u8:
+ * min(n, cap) rows of x1 y1 x2 y2 score location-index to HOST memory, *n = all candidates of the image, *nms_path = 0 if
+ * its NMS ran in shared memory, 1 if in global memory.  Synchronises the device. */
+int w2l_debug_s3fd_candidates(w2l_ctx* ctx, int image, int cap, float* out_host, int* n, int* nms_path);
 
 /* ---- training step (scope row f1): wav2lip_train.py:210-231, color_syncnet_train.py:146-163, hq_wav2lip_train.py:213-255 ----
  * Train-mode forward (BatchNorm on batch statistics over the T*B flatten, conv.py:8-11 / wav2lip.py:93-94; running

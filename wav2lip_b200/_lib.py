@@ -33,6 +33,7 @@ EXPORTS = [
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
     "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
+    "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates",
 ]
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
 WG_PLAIN, WG_STRIDED, WG_TRANSPOSED, WG_SWAP, WG_FOLDED = 0, 1, 2, 3, 4
@@ -151,6 +152,8 @@ def get_lib() -> C.CDLL:
     f32 = C.c_float
     lib.w2l_s3fd_out_dims.argtypes = [i32, i32, C.POINTER(i32)]
     lib.w2l_s3fd_forward.argtypes = [vp, vp, C.POINTER(vp), i32, i32, i32, vp]
+    lib.w2l_s3fd_detect_u8.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, C.POINTER(vp), vp]
+    lib.w2l_debug_s3fd_candidates.argtypes = [vp, i32, i32, vp, C.POINTER(i32), C.POINTER(i32)]
     lib.w2l_crop_resize_u8.argtypes = [vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_paste_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_lipsync_frames_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
@@ -266,6 +269,18 @@ class Context:
                                               None, None, None, None, C.c_void_p(stream)))
         torch.cuda.synchronize(self.device)
         return out
+
+    def s3fd_candidates(self, image: int, cap: int = None):
+        """The sorted pre-NMS candidates (score > 0.5) of one image of the last S3FD detection as a float32 (n, 6) array
+        (x1, y1, x2, y2, score, location index), and which NMS path ran (0: shared memory, 1: global).  Synchronises."""
+        import numpy as np
+        n, path = C.c_int32(), C.c_int32()
+        check(self.lib.w2l_debug_s3fd_candidates(self.h, int(image), 0, None, C.byref(n), C.byref(path)))
+        k = n.value if cap is None else min(int(cap), n.value)
+        out = np.zeros((max(k, 1), 6), dtype=np.float32)
+        check(self.lib.w2l_debug_s3fd_candidates(self.h, int(image), k, C.c_void_p(out.ctypes.data), C.byref(n),
+                                                 C.byref(path)))
+        return out[:k], int(path.value)
 
     def load_weights(self, net: int, tensors: dict, stream: int = 0):
         """tensors: name -> (device_ptr, numel) of fp32 contiguous CUDA tensors."""

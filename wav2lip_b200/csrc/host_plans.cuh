@@ -280,6 +280,51 @@ static int build_s3fd_plan(w2l_ctx* ctx, Plan* pl) {
     return W2L_OK;
 }
 
+// Detection on an S3FD plan: the select / NMS kernels read the fp32 head outputs the plan already writes (found through its
+// export ops); their workspace is allocated once per plan, sized for every anchor of every image.
+static int ensure_s3fd_detect(w2l_ctx* ctx, Plan* pl) {
+    if (pl->det) return W2L_OK;
+    std::unique_ptr<S3fdDetWork> dw(new S3fdDetWork());
+    S3fdDetParams& p = dw->p;
+    memset(&p, 0, sizeof(p));
+    int found = 0;
+    for (const Op& op : pl->ops) {
+        if (op.type != OP_S3FD_EXPORT) continue;
+        S3fdScale& sc = p.sc[op.aux_out / 2];
+        if (op.aux_out % 2 == 0) sc.cls = op.sp_f32; else sc.reg = op.sp_f32;
+        sc.h = op.sp_H; sc.w = op.sp_W;
+        ++found;
+    }
+    if (found != 12) return fail(W2L_ESTATE, "S3FD plan has %d head outputs, expected 12", found);
+    int L = 0;
+    for (int i = 0; i < 6; ++i) { p.sc[i].first = L; L += p.sc[i].h * p.sc[i].w; }
+    const int B = pl->N;
+    p.B = B; p.L = L;
+    p.Lpad = 1;
+    while (p.Lpad < L) p.Lpad <<= 1;
+    p.nchunk = (L + kSelChunk - 1) / kSelChunk;
+    void* q;
+    CKR(plan_alloc(pl, &q, (size_t)B * p.nchunk * 4)); p.chunk_count = (int*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * 4)); p.ncand = (int*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * L * 16)); p.cbox = (float4*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * L * 4)); p.cloc = (int*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * p.Lpad * 8)); p.keys = (uint64_t*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * L)); p.sup = (uint8_t*)q;
+    CKR(plan_alloc(pl, &q, (size_t)B * 4)); p.path = (int*)q;
+    CK(cudaFuncSetAttribute(s3fd_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kNmsSmemBytes));
+    pl->det = std::move(dw);
+    return W2L_OK;
+}
+
+// arguments of a detection replay of an S3FD plan (w2l_s3fd_detect_u8)
+struct S3fdRun {
+    const uint8_t* frames;  // (B, H, W, 3) uint8 on the device
+    int reverse;            // 1: frames are RGB
+    int max_det;
+    float* dets;            // (B, max_det, 5)
+    int32_t* counts;        // (B)
+};
+
 static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, int W = 0) {
     char key[96];
     snprintf(key, sizeof(key), "%d:%d:%d:%d:%d:%d", net, B, T, (int)ctx->keep_all, H, W);
@@ -318,7 +363,7 @@ static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, 
 }
 
 static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, void* out0, void* out1, cudaStream_t st,
-                    bool u8 = false, float* const* outs = nullptr) {
+                    bool u8 = false, float* const* outs = nullptr, const S3fdRun* det = nullptr) {
     const bool side = pl->has_side && ctx->use_side;
     cudaStream_t main_st = st;
     if (side) {
@@ -333,6 +378,18 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
         st = (side && op.lane == 1) ? ctx->s_side : main_st;
         switch (op.type) {
             case OP_INGEST: {
+                if (det) {  // S3FD detection: uint8 frames, mean subtraction (and RGB -> BGR) fused into the ingest
+                    S3fdIngestParams sp;
+                    sp.src = det->frames; sp.dst = op.ip.dst;
+                    sp.N = op.ip.N; sp.H = op.ip.H; sp.W = op.ip.W; sp.Cpad = op.ip.Cpad; sp.Wp = op.ip.Wp; sp.x_off = op.ip.x_off;
+                    sp.Cpix = op.ip.Cpix; sp.lo_off = op.ip.lo_off; sp.reverse = det->reverse;
+                    const long long tot = (long long)sp.N * sp.H * sp.W;
+                    const int blk = (int)std::min<long long>((tot + 255) / 256, ctx->num_sms * 16);
+                    if (ctx->bf16) s3fd_ingest_u8_kernel<true><<<blk, 256, 0, st>>>(sp);
+                    else s3fd_ingest_u8_kernel<false><<<blk, 256, 0, st>>>(sp);
+                    ctx->launches++;
+                    break;
+                }
                 if (u8 && op.ingest_src == 1) {  // uint8 crops: mask + concat + /255 fused into the ingest
                     IngestU8Params up;
                     up.src = (const unsigned char*)in1; up.dst = op.ip.dst;
@@ -391,6 +448,7 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
                 break;
             }
             case OP_S3FD_EXPORT: {
+                if (!outs && det) break;   // detection without the maps
                 if (!outs) return fail(W2L_EINVAL, "S3FD plan needs its 12 output pointers");
                 const long long total = (long long)op.sp_N * op.sp_Cout * op.sp_H * op.sp_W;
                 const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
@@ -407,6 +465,16 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
             }
         }
     }
+    if (det) {
+        S3fdDetParams p = pl->det->p;
+        p.max_det = det->max_det; p.dets = det->dets; p.counts = det->counts;
+        const dim3 grid(p.nchunk, p.B);
+        s3fd_count_kernel<<<grid, kSelChunk, 0, main_st>>>(p);
+        s3fd_select_kernel<<<grid, kSelChunk, 0, main_st>>>(p);
+        s3fd_nms_kernel<<<p.B, kNmsThreads, kNmsSmemBytes, main_st>>>(p);
+        ctx->launches += 3;
+    }
+    if (pl->det) pl->det->last = det != nullptr;
     CK(cudaGetLastError());
     ctx->last_plan[pl->net] = pl;
     return W2L_OK;

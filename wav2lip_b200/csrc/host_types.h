@@ -148,6 +148,12 @@ struct Op {
     bool join_side = false;  // wait for the side stream before this op
 };
 
+// detection work of an S3FD plan (s3fd_detect.cuh), added the first time the plan is used for detection
+struct S3fdDetWork {
+    S3fdDetParams p;       // head pointers, sizes and workspace; max_det / dets / counts are set per call
+    bool last = false;     // the plan's last replay was a detection (its candidates are readable)
+};
+
 struct Plan {
     int net = 0, B = 0, T = 0, N = 0;
     int H = 0, W = 0;              // S3FD: image size
@@ -158,6 +164,7 @@ struct Plan {
     long long last_used = 0;       // LRU stamp
     bool x2 = false;               // split-operand precision: activations carry hi and lo planes
     bool has_side = false;         // some ops run on the side stream
+    std::unique_ptr<S3fdDetWork> det;  // S3FD: detection workspace (nullptr until the first w2l_s3fd_detect_u8)
 };
 
 struct FoldJob { const float* bias; int cout, reps, n_pad; float* scale; float* shift; };  // nonorm blocks: shift = conv bias

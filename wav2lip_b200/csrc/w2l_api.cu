@@ -25,6 +25,7 @@
 #include "mel.cuh"
 #include "netspec.h"
 #include "resize.cuh"
+#include "s3fd_detect.cuh"
 #include "train_kernels.cuh"
 #include "wgrad.cuh"
 
@@ -443,6 +444,57 @@ int w2l_s3fd_forward(w2l_ctx* ctx, const float* img, float* const* outs, int B, 
     Plan* pl;
     CKR(get_plan(ctx, W2L_NET_S3FD, B, 0, &pl, H, W));
     return run_plan(ctx, pl, img, nullptr, nullptr, nullptr, (cudaStream_t)stream, false, outs);
+}
+
+int w2l_s3fd_detect_u8(w2l_ctx* ctx, const uint8_t* frames, int B, int H, int W, int reverse_channels, int max_det, float* dets,
+                       int32_t* counts, float* const* outs, void* stream) {
+    if (!ctx || !frames || !dets || !counts) return fail(W2L_EINVAL, "null argument");
+    if (outs)
+        for (int i = 0; i < 12; ++i) if (!outs[i]) return fail(W2L_EINVAL, "null output %d", i);
+    if (B <= 0 || H < 32 || W < 32) return fail(W2L_EINVAL, "bad shape B=%d H=%d W=%d", B, H, W);
+    if (reverse_channels != 0 && reverse_channels != 1) return fail(W2L_EINVAL, "reverse_channels must be 0 or 1");
+    if (max_det < 1) return fail(W2L_EINVAL, "max_det must be at least 1, got %d", max_det);
+    DeviceGuard g(ctx->device);
+    Plan* pl;
+    CKR(get_plan(ctx, W2L_NET_S3FD, B, 0, &pl, H, W));
+    CKR(ensure_s3fd_detect(ctx, pl));
+    const S3fdRun run{frames, reverse_channels, max_det, dets, counts};
+    return run_plan(ctx, pl, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream, false, outs, &run);
+}
+
+int w2l_debug_s3fd_candidates(w2l_ctx* ctx, int image, int cap, float* out, int* n, int* nms_path) {
+    if (!ctx) return fail(W2L_EINVAL, "null ctx");
+    Plan* pl = ctx->last_plan[W2L_NET_S3FD];
+    if (!pl || !pl->det || !pl->det->last) return fail(W2L_ESTATE, "the last S3FD call was not a detection");
+    const S3fdDetParams& p = pl->det->p;
+    if (image < 0 || image >= p.B) return fail(W2L_EINVAL, "image %d out of range (%d images)", image, p.B);
+    if (cap < 0 || (cap > 0 && !out)) return fail(W2L_EINVAL, "bad output buffer");
+    DeviceGuard g(ctx->device);
+    CK(cudaDeviceSynchronize());
+    int cnt = 0, path = 0;
+    CK(cudaMemcpy(&cnt, p.ncand + image, 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&path, p.path + image, 4, cudaMemcpyDeviceToHost));
+    if (n) *n = cnt;
+    if (nms_path) *nms_path = path;
+    const int k = std::min(cnt, cap);
+    if (k > 0) {
+        std::vector<uint64_t> keys(k);
+        std::vector<float4> box(cnt);
+        std::vector<int> loc(cnt);
+        CK(cudaMemcpy(keys.data(), p.keys + (size_t)image * p.Lpad, (size_t)k * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(box.data(), p.cbox + (size_t)image * p.L, (size_t)cnt * 16, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(loc.data(), p.cloc + (size_t)image * p.L, (size_t)cnt * 4, cudaMemcpyDeviceToHost));
+        for (int r = 0; r < k; ++r) {
+            const uint32_t slot = (uint32_t)keys[r];
+            if (slot >= (uint32_t)cnt) return fail(W2L_ESTATE, "sorted candidate %d refers to slot %u of %d", r, slot, cnt);
+            const uint32_t sb = (uint32_t)(keys[r] >> 32);
+            float sc;
+            memcpy(&sc, &sb, 4);
+            float* o = out + (size_t)r * 6;
+            o[0] = box[slot].x; o[1] = box[slot].y; o[2] = box[slot].z; o[3] = box[slot].w; o[4] = sc; o[5] = (float)loc[slot];
+        }
+    }
+    return W2L_OK;
 }
 
 int w2l_syncnet_forward(w2l_ctx* ctx, const float* mel, const float* face, float* a_emb, float* v_emb, int B, void* stream) {

@@ -65,3 +65,44 @@ class s3fd(_NativeNet):
         _lib.check(ctx.lib.w2l_s3fd_forward(ctx.h, self._p(img), ptrs, B, H, W, C.c_void_p(stream)))
         self._range_guard(ctx, stream)
         return outs
+
+    @staticmethod
+    def num_anchors(H: int, W: int) -> int:
+        """Locations of the six maps of an H x W image (the most boxes a detection can keep)."""
+        dims = (C.c_int32 * 12)()
+        _lib.check(_lib.get_lib().w2l_s3fd_out_dims(int(H), int(W), dims))
+        return sum(dims[2 * i] * dims[2 * i + 1] for i in range(6))
+
+    def detect_u8(self, frames: torch.Tensor, max_det: int, reverse_channels: bool = False, return_maps: bool = False):
+        """The detector on the device (`w2l_s3fd_detect_u8`): frames (B,H,W,3) uint8 CUDA tensor in the order
+        `detect_from_batch` takes them (reverse_channels: reversed first, as api.py:64 does) -> dets (B,max_det,5) float32
+        (x1, y1, x2, y2, score; the first counts[b] rows are image b's boxes, best first, the rest zero), counts (B,)
+        int32, and with return_maps the 12 maps `forward` returns for the same frames."""
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise TypeError(f"expected a uint8 torch tensor, got {getattr(frames, 'dtype', type(frames))}")
+        if frames.dim() != 4 or frames.shape[3] != 3 or frames.shape[1] < 32 or frames.shape[2] < 32:
+            raise ValueError(f"expected (B,H,W,3) with H, W >= 32, got {tuple(frames.shape)}")
+        if isinstance(max_det, bool) or not isinstance(max_det, int) or max_det < 1:
+            raise ValueError(f"max_det must be an int >= 1, got {max_det!r}")
+        ctx = self._ensure(frames)
+        self._same_device(ctx, frames)
+        frames = frames.contiguous()
+        B, H, W, _ = frames.shape
+        dets = torch.empty((B, max_det, 5), device=frames.device, dtype=torch.float32)   # the NMS kernel zero-fills the tail
+        counts = torch.zeros((B,), device=frames.device, dtype=torch.int32)
+        outs, ptrs = None, None
+        if return_maps:
+            dims = (C.c_int32 * 12)()
+            _lib.check(ctx.lib.w2l_s3fd_out_dims(H, W, dims))
+            outs = []
+            for i in range(6):
+                for c in (2, 4):
+                    outs.append(torch.empty((B, c, dims[2 * i], dims[2 * i + 1]), device=frames.device, dtype=torch.float32))
+            ptrs = (C.c_void_p * 12)(*[o.data_ptr() for o in outs])
+        if B == 0:
+            return dets, counts, outs
+        stream = torch.cuda.current_stream(frames.device).cuda_stream
+        _lib.check(ctx.lib.w2l_s3fd_detect_u8(ctx.h, self._p(frames), B, H, W, 1 if reverse_channels else 0, max_det,
+                                              self._p(dets), self._p(counts), ptrs, C.c_void_p(stream)))
+        self._range_guard(ctx, stream)
+        return dets, counts, outs

@@ -83,3 +83,23 @@ class SFDDetector:
             d = d[nms(d, 0.3), :]
             out.append([r for r in d if r[-1] > 0.5])
         return out
+
+    def detect_from_batch_u8(self, images, max_det=None, reverse_channels=False):
+        """`detect_from_batch` on the device: images (B,H,W,3) uint8 BGR, a CUDA tensor or host memory (copied to the
+        device once, as uint8) -> per image a float32 (k, 5) array of x1, y1, x2, y2, score, best first, at most max_det
+        rows (None: every box).  The content is `detect_from_batch`'s, up to the order of exactly tied scores (the larger
+        location index first, DESIGN.md §3.6)."""
+        x = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(images)))
+        if x.dtype != torch.uint8:
+            raise TypeError(f"expected uint8 frames, got {x.dtype}")
+        if x.dim() != 4 or x.shape[3] != 3:
+            raise ValueError(f"expected (B,H,W,3) frames, got {tuple(x.shape)}")
+        if not x.is_cuda:
+            x = x.to(self.device)
+        if max_det is None:
+            max_det = self.face_detector.num_anchors(x.shape[1], x.shape[2])
+        with torch.no_grad():
+            dets, counts, _ = self.face_detector.detect_u8(x, max_det, reverse_channels=reverse_channels)
+        counts = counts.cpu().numpy()
+        dets = dets[:, :int(counts.max(initial=0))].cpu().numpy()   # only the rows that hold boxes cross to the host
+        return [dets[i, :counts[i]].copy() for i in range(dets.shape[0])]
