@@ -1,4 +1,4 @@
-"""The training loops of the reference on the H100 core, with synthetic batches (there is no dataset here):
+"""The training loops of the reference on the H100 core, on synthetic batches or a preprocessed dataset:
 
   --mode script   the statements of wav2lip_train.py:210-231 as the script writes them — `model.train()`, `g = model(indiv_mels, x)`,
                   `get_sync_loss` through the frozen expert (left in train mode, :187-189), `recon_loss`, `loss.backward()`,
@@ -9,7 +9,12 @@
   --mode hq       hq_wav2lip_train.py:213-255: generator + perceptual loss through the quality discriminator + the
                   discriminator's real/fake step, two Adam optimizers (betas 0.5, 0.999), through the autograd bridge.
 
+With --data-root DIR (a preprocess.py-layout dataset) the batches are the reference Dataset's, assembled on the device from a
+cache built once (wav2lip_b200/data.py: TrainDataCache + Wav2LipBatches); the video list is filelists/train.txt relative to the
+current directory, as hparams.get_image_list reads it, or --filelist F.  Without it the batches are synthetic.
+
 Run:  python examples/train_loop.py --mode fused --iters 20 --batch 16
+      python examples/train_loop.py --mode fused --data-root DIR [--filelist F]
       python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/train_loop.py --mode fused
 """
 import argparse
@@ -45,6 +50,8 @@ def main():
     ap.add_argument("--mode", choices=["script", "fused", "hq"], default="fused")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--batch", type=int, default=16)
+    ap.add_argument("--data-root", default=None, help="train on this preprocessed dataset instead of synthetic batches")
+    ap.add_argument("--filelist", default=None, help="video list (default: filelists/train.txt in the current directory)")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
@@ -77,11 +84,22 @@ def main():
         optimizer = optim.Adam([p for p in model.parameters() if p.requires_grad], lr=1e-4, betas=(0.5, 0.999))
         disc_optimizer = optim.Adam([p for p in disc.parameters() if p.requires_grad], lr=1e-4, betas=(0.5, 0.999))
 
+    feed = None
+    if args.data_root is not None:
+        from wav2lip_b200.data import TrainDataCache, Wav2LipBatches
+        cache = TrainDataCache.from_data_root(args.data_root, "train", filelist=args.filelist, device=dev)
+        feed = Wav2LipBatches(cache, args.batch)
+        if rank == 0:
+            print(f"dataset: {len(cache.videos)} videos, {cache.n_frames} frames, {cache.n_mel_rows} mel rows", flush=True)
+
     t0 = None
     for it in range(args.iters):
         if it == 2:
             torch.cuda.synchronize(); t0 = time.time()
-        x, indiv_mels, mel, gt = batch(args.batch, dev, seed=1000 * rank + it)
+        if feed is not None:
+            x, indiv_mels, mel, gt = feed.next_batch()
+        else:
+            x, indiv_mels, mel, gt = batch(args.batch, dev, seed=1000 * rank + it)
         if args.mode == "fused":
             sync_loss, l1, _, loss = step(x, indiv_mels, mel, gt).tolist()
         elif args.mode == "script":

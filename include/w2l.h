@@ -140,6 +140,23 @@ int w2l_paste_u8(w2l_ctx* ctx, const uint8_t* pred_dev, const uint8_t* frames_de
 int w2l_lipsync_frames_u8(w2l_ctx* ctx, const float* mel_dev, const uint8_t* frames_dev, int F, int H, int W,
                           const int32_t* boxes_host, int N, uint8_t* out_frames_dev, void* stream);
 
+/* Scope row (f3): the training scripts' batch assembly, `default_collate` of B `Dataset.__getitem__` calls
+ * (wav2lip_train.py:111-164, identical in hq_wav2lip_train.py; color_syncnet_train.py:69-131) from a cache, in one launch.
+ *   frames (n_frames,96,96,3) uint8 BGR = cv2.resize(cv2.imread(f), (96, 96)) (wav2lip_train.py:63-70); mels (n_mel_rows,80) fp32
+ *   = every video's `audio.melspectrogram(wav).T` (:138-141) stacked.  Both in device or pinned host memory; pageable is refused.
+ *   samples_host: B rows of int32 in HOST memory, validated before any launch (slot < n_frames, row + 16 <= end <= n_mel_rows,
+ *   label 0 / 1).  Mel rows are absolute cache rows, `end` is the row after the sample's video.
+ *   Pixels are float32(u / 255.) with the division in float64 (prepare_window, :101-106).  Outputs: 16-byte aligned device memory.
+ * w2l_train_batch_wav2lip   rows of 17: window slots[5], wrong-window slots[5], mel row, indiv rows[5], end
+ *                           -> x (B,6,5,96,96) (channels 0-2 the window with rows 48-95 zeroed, :152-157), indiv_mels (B,5,1,80,16)
+ *                           (get_segmented_mels, :88-99), mel (B,1,80,16) (crop_audio_window, :75-86), gt (B,3,5,96,96) (:154)
+ * w2l_train_batch_syncnet   rows of 8: window slots[5], mel row, label, end
+ *                           -> x (B,15,48,96) (channel 3t+c, rows 48-95: color_syncnet_train.py:123-126), mel (B,1,80,16), y (B,1) */
+int w2l_train_batch_wav2lip(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frames, const float* mels, int64_t n_mel_rows,
+                            const int32_t* samples_host, int B, float* x, float* indiv_mels, float* mel, float* gt, void* stream);
+int w2l_train_batch_syncnet(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frames, const float* mels, int64_t n_mel_rows,
+                            const int32_t* samples_host, int B, float* x, float* mel, float* y, void* stream);
+
 /* Scope row (f4): the S3FD face detector's network (face_detection/detection/sfd/net_s3fd.py:22-129), the per-frame GPU
  * work of inference.py's face_detect (:73-100): 19 conv+ReLU layers (VGG16 backbone + fc6/fc7 + conv6/7), 5 max-pools,
  * 3 L2Norm layers and the 12 mbox heads, max-out of the first scale's background logits included.

@@ -33,7 +33,7 @@ EXPORTS = [
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
     "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
-    "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates",
+    "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
 ]
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
 WG_PLAIN, WG_STRIDED, WG_TRANSPOSED, WG_SWAP, WG_FOLDED = 0, 1, 2, 3, 4
@@ -157,6 +157,8 @@ def get_lib() -> C.CDLL:
     lib.w2l_crop_resize_u8.argtypes = [vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_paste_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_lipsync_frames_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
+    lib.w2l_train_batch_wav2lip.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, vp, vp, vp, vp]
+    lib.w2l_train_batch_syncnet.argtypes = [vp, vp, i64, vp, i64, vp, i32, vp, vp, vp, vp]
     lib.w2l_train_bind.argtypes = [vp, i32, i32, C.POINTER(cp), C.POINTER(vp), C.POINTER(vp), C.POINTER(i64)]
     lib.w2l_train_forward.argtypes = [vp, i32, vp, vp, vp, vp, i32, i32, i32, vp]
     lib.w2l_train_backward.argtypes = [vp, i32, vp, vp, vp, i32, vp]

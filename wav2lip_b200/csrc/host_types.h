@@ -207,6 +207,7 @@ struct w2l_ctx {
     cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
     void* stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     int* boxes_dev = nullptr; int box_cap = 0;                 // crop / paste boxes (row f2)
+    int* samples_dev = nullptr; size_t sample_cap = 0;         // training-batch sample table (ints)
     uint8_t *crops_dev = nullptr, *preds_dev = nullptr; size_t crop_cap = 0;
     float* scratch = nullptr;  // partial sums of the loss kernels
     size_t scratch_bytes = 0;

@@ -8,10 +8,12 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <dlfcn.h>
 #include <functional>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <string>
@@ -26,6 +28,7 @@
 #include "netspec.h"
 #include "resize.cuh"
 #include "s3fd_detect.cuh"
+#include "train_data.cuh"
 #include "train_kernels.cuh"
 #include "wgrad.cuh"
 
@@ -155,6 +158,7 @@ int w2l_destroy(w2l_ctx* ctx) {
     for (int i = 0; i < 2; ++i) { if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]); if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]); if (ctx->ev_out[i]) cudaEventDestroy(ctx->ev_out[i]); }
     if (ctx->scratch) cudaFree(ctx->scratch);
     if (ctx->boxes_dev) cudaFree(ctx->boxes_dev);
+    if (ctx->samples_dev) cudaFree(ctx->samples_dev);
     if (ctx->crops_dev) cudaFree(ctx->crops_dev);
     if (ctx->preds_dev) cudaFree(ctx->preds_dev);
     if (ctx->mel_tw) cudaFree(ctx->mel_tw);
@@ -421,6 +425,101 @@ int w2l_lipsync_frames_u8(w2l_ctx* ctx, const float* mel, const uint8_t* frames,
     CKR(w2l_generator_forward_u8(ctx, mel, ctx->crops_dev, ctx->preds_dev, N, stream));
     const long long total = (long long)N * H * W;
     paste_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 32), 256, 0, st>>>(ctx->preds_dev, 96, frames, H, W, ctx->boxes_dev, N, out_frames);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return W2L_OK;
+}
+
+
+// ---- scope row f3: the training scripts' Dataset.__getitem__ + default_collate, one gather per batch ----
+// The gather reads the cache through `p` itself: device (or managed) memory of this context's device, or page-locked host
+// memory, which unified addressing maps at the same address.  Pageable memory cannot be read by a kernel.
+static int train_source(w2l_ctx* ctx, const void* p, const char* what, const void** dev) {
+    cudaPointerAttributes a;
+    cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(W2L_EINVAL, "%s: cudaPointerGetAttributes: %s", what, cudaGetErrorString(e)); }
+    if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) {
+        if (a.type == cudaMemoryTypeDevice && a.device != ctx->device)
+            return fail(W2L_EINVAL, "%s is on device %d, the context on device %d", what, a.device, ctx->device);
+        *dev = p;
+        return W2L_OK;
+    }
+    if (a.type == cudaMemoryTypeHost && a.devicePointer) { *dev = a.devicePointer; return W2L_OK; }
+    return fail(W2L_EINVAL, "%s is pageable host memory: the batch gather reads device or pinned (page-locked) memory only", what);
+}
+
+// every row of the host sample table, before anything touches the device
+static int check_samples(const int32_t* s, int B, int fields, int n_slots, int mel_at, int n_mel, int label_at,
+                         int64_t n_frames, int64_t n_mel_rows) {
+    for (int b = 0; b < B; ++b) {
+        const int32_t* r = s + (size_t)b * fields;
+        for (int k = 0; k < n_slots; ++k)
+            if (r[k] < 0 || r[k] >= n_frames) return fail(W2L_EINVAL, "sample %d: frame slot %d is outside the %lld cached frames", b, r[k], (long long)n_frames);
+        const int32_t end = r[fields - 1];
+        if (end > n_mel_rows) return fail(W2L_EINVAL, "sample %d: video end row %d is past the %lld cached mel rows", b, end, (long long)n_mel_rows);
+        for (int k = 0; k < n_mel; ++k)
+            if (r[mel_at + k] < 0 || (int64_t)r[mel_at + k] + 16 > end)
+                return fail(W2L_EINVAL, "sample %d: mel window at row %d does not end by its video's end row %d", b, r[mel_at + k], end);
+        if (label_at >= 0 && r[label_at] != 0 && r[label_at] != 1) return fail(W2L_EINVAL, "sample %d: label %d is not 0 or 1", b, r[label_at]);
+    }
+    return W2L_OK;
+}
+
+// argument checks shared by both entries: host-side ones first (no context needed), then the two cache pointers
+static int train_batch_args(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frames, const float* mels, int64_t n_mel_rows,
+                            const int32_t* samples, int B, std::initializer_list<const void*> outs, int fields, int n_slots,
+                            int mel_at, int n_mel, int label_at, const void** fdev, const void** mdev) {
+    if (!frames || !mels || !samples) return fail(W2L_EINVAL, "null argument");
+    for (const void* o : outs)
+        if (!o || ((uintptr_t)o & 15)) return fail(W2L_EINVAL, "outputs must be non-null and 16-byte aligned");
+    if (B <= 0 || n_frames <= 0 || n_mel_rows < 16 || n_mel_rows > INT32_MAX)
+        return fail(W2L_EINVAL, "bad batch %d / %lld frames / %lld mel rows", B, (long long)n_frames, (long long)n_mel_rows);
+    CKR(check_samples(samples, B, fields, n_slots, mel_at, n_mel, label_at, n_frames, n_mel_rows));
+    if (!ctx) return fail(W2L_EINVAL, "null context");
+    CKR(train_source(ctx, frames, "frames", fdev));
+    return train_source(ctx, mels, "mels", mdev);
+}
+
+static int upload_samples(w2l_ctx* ctx, const int32_t* s, size_t n, cudaStream_t st) {
+    if (ctx->sample_cap < n) {
+        CK(cudaDeviceSynchronize());
+        if (ctx->samples_dev) cudaFree(ctx->samples_dev);
+        ctx->samples_dev = nullptr; ctx->sample_cap = 0;
+        void* p = nullptr;
+        CKR(dev_alloc(&p, n * 4));
+        ctx->samples_dev = (int*)p; ctx->sample_cap = n;
+    }
+    CK(cudaMemcpyAsync(ctx->samples_dev, s, n * 4, cudaMemcpyHostToDevice, st));
+    return W2L_OK;
+}
+
+int w2l_train_batch_wav2lip(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frames, const float* mels, int64_t n_mel_rows,
+                            const int32_t* samples_host, int B, float* x, float* indiv_mels, float* mel, float* gt, void* stream) {
+    const void *fd = nullptr, *md = nullptr;
+    CKR(train_batch_args(ctx, frames, n_frames, mels, n_mel_rows, samples_host, B, {x, indiv_mels, mel, gt},
+                         TD_W2L_FIELDS, 10, 10, 6, -1, &fd, &md));
+    DeviceGuard g(ctx->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    CKR(upload_samples(ctx, samples_host, (size_t)B * TD_W2L_FIELDS, st));
+    const long long total = (long long)B * (2 * 5 * 96 * 24 + 6 * 80 * 4);
+    train_batch_wav2lip_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16), 256, 0, st>>>(
+        (const uint8_t*)fd, (const float*)md, ctx->samples_dev, B, x, indiv_mels, mel, gt);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return W2L_OK;
+}
+
+int w2l_train_batch_syncnet(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frames, const float* mels, int64_t n_mel_rows,
+                            const int32_t* samples_host, int B, float* x, float* mel, float* y, void* stream) {
+    const void *fd = nullptr, *md = nullptr;
+    CKR(train_batch_args(ctx, frames, n_frames, mels, n_mel_rows, samples_host, B, {x, mel, y},
+                         TD_SYNC_FIELDS, 5, 5, 1, 6, &fd, &md));
+    DeviceGuard g(ctx->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    CKR(upload_samples(ctx, samples_host, (size_t)B * TD_SYNC_FIELDS, st));
+    const long long total = (long long)B * (5 * 48 * 24 + 80 * 4);
+    train_batch_syncnet_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16), 256, 0, st>>>(
+        (const uint8_t*)fd, (const float*)md, ctx->samples_dev, B, x, mel, y);
     ctx->launches++;
     CK(cudaGetLastError());
     return W2L_OK;
