@@ -314,6 +314,29 @@ int w2l_adam_step(w2l_ctx* ctx, int net, float lr, float beta1, float beta2, flo
  *   [sync_loss, l1, 0, loss] or NULL. */
 int w2l_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels_dev, const float* x_dev, const float* mel_dev,
                            const float* gt_dev, int B, int T, float syncnet_wt, float lr, float* losses_dev, void* stream);
+/* One whole iteration of hq_wav2lip_train.py:212-256 on the bound generator, (frozen, train-mode) expert and
+ * discriminator, all bound to this context (the discriminator's gradients in one contiguous arena):
+ *   g = model(indiv_mels, x); sync_loss if syncnet_wt > 0; perceptual = BCE(disc(g), 1) if disc_wt > 0; l1;
+ *   loss = syncnet_wt*sync + disc_wt*perceptual + (1-syncnet_wt-disc_wt)*l1; backward; Adam(lr, (0.5,0.999), 1e-8);
+ *   then the discriminator: BCE(disc(gt), 1) + BCE(disc(g.detach()), 0), backward, Adam(disc_lr, (0.5,0.999), 1e-8).
+ * The discriminator's forward on g runs once (the value :252 recomputes); its step runs beside the generator's backward.
+ * With a communicator (w2l_comm_init) both networks' gradients are averaged over the ranks.
+ *   inputs as w2l_wav2lip_train_step; losses_dev: 6 floats on the device
+ *   [sync_loss, l1, perceptual, loss, disc_real_loss, disc_fake_loss] or NULL. */
+int w2l_hq_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels_dev, const float* x_dev, const float* mel_dev,
+                              const float* gt_dev, int B, int T, float syncnet_wt, float disc_wt, float lr, float disc_lr,
+                              float* losses_dev, void* stream);
+/* One whole iteration of color_syncnet_train.py:149-163 on the bound expert: a, v = model(mel, x) in train mode;
+ * loss = cosine_loss(a, v, y); backward; [gradient all-reduce, overlapped]; Adam(lr, (0.9,0.999), 1e-8).
+ *   mel (B,1,80,16), x (B,15,48,96), y (B,1) in {0, 1}; loss_dev: 1 float on the device or NULL. */
+int w2l_syncnet_train_step(w2l_ctx* ctx, const float* mel_dev, const float* x_dev, const float* y_dev, int B, float lr,
+                           float* loss_dev, void* stream);
+/* `optimizer.state_dict()` / `optimizer.load_state_dict()` of the fused steps' Adam: the first and second moments of the
+ * n named bound tensors of `net` (each with a gradient; m_ptrs[i] / v_ptrs[i] are fp32 device buffers of the tensor's
+ * size) are copied out of the context (direction 0) or into it (direction 1), and *step, the step count of the bias
+ * correction, is read (0) or set (1).  Before the first step the moments are zero and the count is 0. */
+int w2l_adam_state(w2l_ctx* ctx, int net, int direction, int n, const char* const* names, float* const* m_ptrs,
+                   float* const* v_ptrs, int64_t* step, void* stream);
 /* copies the generator output g (B,3,T,96,96) of the last fused step into out_dev (n floats) */
 int w2l_train_last_output(w2l_ctx* ctx, float* out_dev, int64_t n, void* stream);
 /* algorithmic forward FLOPs of the last training plan of `net` (2 x true MACs of its convs) */

@@ -31,6 +31,7 @@ EXPORTS = [
     "w2l_f16_overflow",
     "w2l_crop_resize_u8", "w2l_paste_u8", "w2l_lipsync_frames_u8", "w2l_s3fd_out_dims", "w2l_s3fd_forward",
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
+    "w2l_hq_wav2lip_train_step", "w2l_syncnet_train_step", "w2l_adam_state",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
     "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
     "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
@@ -165,6 +166,9 @@ def get_lib() -> C.CDLL:
     lib.w2l_adam_step.argtypes = [vp, i32, f32, f32, f32, f32, vp]
     lib.w2l_wav2lip_train_step.argtypes = [vp, vp, vp, vp, vp, i32, i32, f32, f32, vp, vp]
     lib.w2l_train_last_output.argtypes = [vp, vp, i64, vp]
+    lib.w2l_hq_wav2lip_train_step.argtypes = [vp, vp, vp, vp, vp, i32, i32, f32, f32, f32, f32, vp, vp]
+    lib.w2l_syncnet_train_step.argtypes = [vp, vp, vp, vp, i32, f32, vp, vp]
+    lib.w2l_adam_state.argtypes = [vp, i32, i32, i32, C.POINTER(cp), C.POINTER(vp), C.POINTER(vp), C.POINTER(i64), vp]
     lib.w2l_train_flops.argtypes = [vp, i32]
     lib.w2l_train_flops.restype = C.c_double
     lib.w2l_train_profile.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]

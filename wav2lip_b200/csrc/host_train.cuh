@@ -77,7 +77,9 @@ struct TrainPlan {
     double fwd_flops = 0;
 };
 
-struct AdamSlot { std::vector<float*> m, v; std::vector<AdamTensor> host; AdamTensor* dev = nullptr; long long step = 0; };
+// Adam moments of one net's bound tensors that have a gradient, in the order of the name map (alphabetical): names[i] owns
+// host[i]; step is the count the bias correction uses (torch.optim.Adam's state['step'])
+struct AdamSlot { std::vector<std::string> names; std::vector<float*> m, v; std::vector<AdamTensor> host; AdamTensor* dev = nullptr; long long step = 0; };
 
 // NCCL entry points resolved at run time from the libnccl.so.2 that torch already loaded (no link-time dependency)
 typedef int (*NcclGetUniqueIdFn)(void*);
@@ -97,7 +99,7 @@ struct TrainState {
     float* loss_dev = nullptr;     // [8]
     float *a_emb = nullptr, *v_emb = nullptr, *da = nullptr, *dv = nullptr; int emb_cap = 0;
     float* g_buf = nullptr; float* dg_buf = nullptr; size_t g_cap = 0;
-    float *prob = nullptr, *dprob = nullptr; int prob_cap = 0;
+    float *prob = nullptr, *dprob = nullptr; int prob_cap = 0;   // disc probabilities on g | gt (2N), their gradients (3N)
     // data-parallel gradient all-reduce
     void* nccl_lib = nullptr; void* comm = nullptr; int rank = 0, world = 1;
     NcclAllReduceFn all_reduce = nullptr; NcclCommDestroyFn comm_destroy = nullptr; NcclGetErrorStringFn err_string = nullptr;
@@ -108,6 +110,8 @@ struct TrainState {
     cudaStream_t s_wg = nullptr; cudaEvent_t ev_dz = nullptr, ev_wg = nullptr, ev_wgb = nullptr;
     // the audio encoder (small, latency-bound launches) runs beside the face encoder, forward and backward
     cudaStream_t s_aux = nullptr; cudaEvent_t ev_aux_fork = nullptr, ev_aux_join = nullptr;
+    // the discriminator's step of the hq iteration (its two backward passes, all-reduce, Adam) beside the generator's backward
+    cudaStream_t s_disc = nullptr; cudaEvent_t ev_disc_fork = nullptr, ev_disc_join = nullptr;
     std::vector<w2l_train_block_info> last_block_info;   // the block of the last w2l_conv_block_train (its plan is freed)
 };
 
@@ -138,8 +142,10 @@ static void free_train_state(w2l_ctx* ctx) {
     if (ts->ev_bucket) cudaEventDestroy(ts->ev_bucket);
     if (ts->ev_comm) cudaEventDestroy(ts->ev_comm);
     if (ts->s_wg) cudaStreamDestroy(ts->s_wg);
-    for (cudaEvent_t e : {ts->ev_dz, ts->ev_wg, ts->ev_wgb, ts->ev_aux_fork, ts->ev_aux_join}) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : {ts->ev_dz, ts->ev_wg, ts->ev_wgb, ts->ev_aux_fork, ts->ev_aux_join, ts->ev_disc_fork, ts->ev_disc_join})
+        if (e) cudaEventDestroy(e);
     if (ts->s_aux) cudaStreamDestroy(ts->s_aux);
+    if (ts->s_disc) cudaStreamDestroy(ts->s_disc);
     delete ts;
     ctx->train = nullptr;
 }
@@ -595,7 +601,10 @@ static int build_disc_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_need, b
     return W2L_OK;
 }
 
-enum : int { TRAIN_WGRAD = 1, TRAIN_ACCUMULATE = 2, TRAIN_INPUT_GRAD = 4, TRAIN_NO_STAT_UPDATE = 8 };
+enum : int { TRAIN_WGRAD = 1, TRAIN_ACCUMULATE = 2, TRAIN_INPUT_GRAD = 4, TRAIN_NO_STAT_UPDATE = 8,   // = W2L_TRAIN_*
+             // passes of the fused steps only:
+             TRAIN_SKIP_INPUT_GRAD = 16,   // a plan built with its input gradient: leave that last dgrad out of this pass
+             TRAIN_ONE_STREAM = 32 };      // every launch on the caller's stream (a lane of its own beside another backward)
 
 static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, bool input_grad, TrainPlan** out) {
     TrainState* ts = train_state(ctx);
@@ -737,6 +746,13 @@ static int ensure_aux_stream(TrainState* ts) {
     CK(cudaEventCreateWithFlags(&ts->ev_aux_join, cudaEventDisableTiming));
     return W2L_OK;
 }
+static int ensure_disc_stream(TrainState* ts) {
+    if (ts->s_disc) return W2L_OK;
+    CK(cudaStreamCreateWithFlags(&ts->s_disc, cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(&ts->ev_disc_fork, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&ts->ev_disc_join, cudaEventDisableTiming));
+    return W2L_OK;
+}
 static bool has_aux_lane(const TrainPlan* tp) {
     for (const TBlock& b : tp->blocks) if (b.lane == 1) return true;
     return false;
@@ -744,7 +760,8 @@ static bool has_aux_lane(const TrainPlan* tp) {
 
 // s_wg != nullptr: the block's wgrad (+ its split-K reduction) goes to that stream, ordered after this block's dz (ev);
 // the caller joins the stream before anything consumes the parameter gradients.
-static int block_backward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool wgrad, bool accumulate, cudaStream_t st,
+//   dgrad == false: the input gradient of this block is not wanted in this pass (TRAIN_SKIP_INPUT_GRAD)
+static int block_backward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool wgrad, bool accumulate, bool dgrad, cudaStream_t st,
                           cudaStream_t s_wg = nullptr, cudaEvent_t ev = nullptr) {
     const int C = b.L.cout;
     ChanReduceParams rp;
@@ -786,7 +803,7 @@ static int block_backward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool wgrad, bo
         CK(cudaStreamWaitEvent(s_wg, ev, 0));
         CKR(launch_wgrad(ctx, tp, b, accumulate, s_wg));
     }
-    for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st));
+    if (dgrad) for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st));
     if (!side && wgrad && b.wg.on) CKR(launch_wgrad(ctx, tp, b, accumulate, st));
     return W2L_OK;
 }
@@ -885,12 +902,16 @@ static int train_backward(w2l_ctx* ctx, TrainPlan* tp, const float* d0, const fl
         disc_head_bwd_kernel<true><<<1, 512, 0, st>>>(tp->feat.ptr(), tp->feat.Cs, hw, tp->prob_out, d0, tp->N, 512, tp->dfeat.ptr(), dw, db, accf);
         ctx->launches++;
     }
+    const bool one_stream = (flags & TRAIN_ONE_STREAM) != 0;
     cudaStream_t s_wg = nullptr;
-    if (wgrad && ctx->use_wg_stream) { CKR(ensure_wg_stream(ts)); s_wg = ts->s_wg; }
+    if (wgrad && ctx->use_wg_stream && !one_stream) { CKR(ensure_wg_stream(ts)); s_wg = ts->s_wg; }
+    // the plan's own input gradient (first block's dx), left out of a pass that only wants parameter gradients
+    const void* skip_dx = nullptr;
+    if ((flags & TRAIN_SKIP_INPUT_GRAD) && tp->input_grad) skip_dx = tp->net == W2L_NET_DISC ? tp->dframes_in.base : tp->dface_in.base;
     // audio-encoder blocks (lane 1): their backward chain starts at the gradient of the audio embedding — produced by
     // face_decoder_blocks.0.0's dgrad (generator) or by the normalisation backward above (SyncNet) — and shares nothing with
     // the face encoder's: it runs on the auxiliary stream, forked at that point, joined before the last block's hook
-    const bool aux = ctx->use_aux_stream && tp->blocks.size() > 1 && has_aux_lane(tp);
+    const bool aux = ctx->use_aux_stream && !one_stream && tp->blocks.size() > 1 && has_aux_lane(tp);
     bool forked = false, waited = false, joined = false;
     if (aux) {
         CKR(ensure_aux_stream(ts));
@@ -913,7 +934,8 @@ static int train_backward(w2l_ctx* ctx, TrainPlan* tp, const float* d0, const fl
             if (!waited) { CK(cudaStreamWaitEvent(ts->s_aux, ts->ev_aux_fork, 0)); waited = true; }
             bs = ts->s_aux;
         }
-        CKR(block_backward(ctx, tp, b, wgrad, acc, bs, s_wg, ts->ev_dz));
+        const bool dgrad = !(skip_dx && b.dx.base == skip_dx);
+        CKR(block_backward(ctx, tp, b, wgrad, acc, dgrad, bs, s_wg, ts->ev_dz));
         if (aux && !forked && b.L.name == "face_decoder_blocks.0.0") { CK(cudaEventRecord(ts->ev_aux_fork, st)); forked = true; }
         if (k == 0) CKR(join_aux());
         if (after_block) CKR((*after_block)(k));
@@ -942,7 +964,10 @@ static int ensure_train_scratch(w2l_ctx* ctx, int B, int T) {
     }
     if (ts->prob_cap < N) {
         CK(cudaDeviceSynchronize());
-        for (float** q : {&ts->prob, &ts->dprob}) { if (*q) cudaFree(*q); CKR(dev_alloc(&p, (size_t)N * 4)); *q = (float*)p; }
+        if (ts->prob) cudaFree(ts->prob);
+        if (ts->dprob) cudaFree(ts->dprob);
+        CKR(dev_alloc(&p, (size_t)2 * N * 4)); ts->prob = (float*)p;
+        CKR(dev_alloc(&p, (size_t)3 * N * 4)); ts->dprob = (float*)p;
         ts->prob_cap = N;
     }
     const size_t gn = (size_t)N * 3 * 9216;
@@ -954,27 +979,35 @@ static int ensure_train_scratch(w2l_ctx* ctx, int B, int T) {
     return W2L_OK;
 }
 
+// the moments (zero) of every bound tensor of `net` that has a gradient, allocated at the first use
+static int ensure_adam_slot(w2l_ctx* ctx, int net, cudaStream_t st) {
+    TrainState* ts = train_state(ctx);
+    AdamSlot& a = ts->adam[net];
+    if (a.dev) return W2L_OK;
+    for (auto& kv : ts->bound[net]) {
+        if (!kv.second.grad) continue;
+        void *m = nullptr, *v = nullptr;
+        CKR(dev_alloc(&m, (size_t)kv.second.n * 4));
+        CKR(dev_alloc(&v, (size_t)kv.second.n * 4));
+        CK(cudaMemsetAsync(m, 0, (size_t)kv.second.n * 4, st));
+        CK(cudaMemsetAsync(v, 0, (size_t)kv.second.n * 4, st));
+        a.names.push_back(kv.first);
+        a.m.push_back((float*)m); a.v.push_back((float*)v);
+        a.host.push_back(AdamTensor{kv.second.value, kv.second.grad, (float*)m, (float*)v, kv.second.n});
+    }
+    if (a.host.empty()) return fail(W2L_ESTATE, "adam: no gradient tensors bound for net %d", net);
+    void* d = nullptr;
+    CKR(dev_alloc(&d, a.host.size() * sizeof(AdamTensor)));
+    a.dev = (AdamTensor*)d;
+    CK(cudaMemcpyAsync(a.dev, a.host.data(), a.host.size() * sizeof(AdamTensor), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    return W2L_OK;
+}
+
 static int adam_step(w2l_ctx* ctx, int net, float lr, float beta1, float beta2, float eps, float grad_scale, cudaStream_t st) {
     TrainState* ts = train_state(ctx);
     AdamSlot& a = ts->adam[net];
-    if (!a.dev) {
-        for (auto& kv : ts->bound[net]) {
-            if (!kv.second.grad) continue;
-            void *m = nullptr, *v = nullptr;
-            CKR(dev_alloc(&m, (size_t)kv.second.n * 4));
-            CKR(dev_alloc(&v, (size_t)kv.second.n * 4));
-            CK(cudaMemsetAsync(m, 0, (size_t)kv.second.n * 4, st));
-            CK(cudaMemsetAsync(v, 0, (size_t)kv.second.n * 4, st));
-            a.m.push_back((float*)m); a.v.push_back((float*)v);
-            a.host.push_back(AdamTensor{kv.second.value, kv.second.grad, (float*)m, (float*)v, kv.second.n});
-        }
-        if (a.host.empty()) return fail(W2L_ESTATE, "adam: no gradient tensors bound for net %d", net);
-        void* d = nullptr;
-        CKR(dev_alloc(&d, a.host.size() * sizeof(AdamTensor)));
-        a.dev = (AdamTensor*)d;
-        CK(cudaMemcpyAsync(a.dev, a.host.data(), a.host.size() * sizeof(AdamTensor), cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));
-    }
+    CKR(ensure_adam_slot(ctx, net, st));
     a.step++;
     AdamParams p;
     p.t = a.dev; p.lr = lr; p.beta1 = beta1; p.beta2 = beta2; p.eps = eps;

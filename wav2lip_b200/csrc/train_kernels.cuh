@@ -467,24 +467,49 @@ __global__ void gen_loss_grad_kernel(const GenLossGradParams p) {
     }
 }
 
-// BCE(pred, target) mean and its gradient wrt pred (hq_wav2lip_train.py:246-252, wav2lip.py:171-172), one block
-__global__ void bce_const_target_kernel(const float* pred, int n, float target, float scale, float* loss, float* dpred) {
-    __shared__ float sh[32];
-    float s = 0.0f;
+// The three BCE terms of hq_wav2lip_train.py:233-252 from the discriminator's probabilities on g (p_fake) and on gt
+// (p_real), n each, in one block (a fixed reduction order: deterministic):
+//   loss[2] = BCE(p_fake, 1) (perceptual, 0 when disc_wt == 0), loss[4] = BCE(p_real, 1), loss[5] = BCE(p_fake, 0)
+//   d_perc = disc_wt * dBCE(p_fake, 1)/dp;   d_fake = dBCE(p_fake, 0)/dp;   d_real = dBCE(p_real, 1)/dp
+// torch's arithmetic: logs clamped at -100, dBCE/dp = (p - t) / max(p (1 - p), 1e-12) / n.
+__global__ void __launch_bounds__(1024) disc_bce_kernel(const float* p_fake, const float* p_real, int n, float disc_wt, float* loss,
+                                                        float* d_perc, float* d_fake, float* d_real) {
+    __shared__ float sh[3][32];
+    float s_perc = 0.0f, s_fake = 0.0f, s_real = 0.0f;
+    const float inv_n = 1.0f / (float)n;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float p = pred[i];
-        s -= target * fmaxf(logf(p), -100.0f) + (1.0f - target) * fmaxf(logf(1.0f - p), -100.0f);
-        if (dpred) dpred[i] = scale / (float)n * (p - target) / fmaxf(p * (1.0f - p), 1e-12f);
+        const float pf = p_fake[i], pr = p_real[i];
+        s_perc -= fmaxf(logf(pf), -100.0f);
+        s_fake -= fmaxf(log1pf(-pf), -100.0f);
+        s_real -= fmaxf(logf(pr), -100.0f);
+        const float qf = fmaxf(pf * (1.0f - pf), 1e-12f), qr = fmaxf(pr * (1.0f - pr), 1e-12f);
+        // (torch's order: grad * (p - t) / max(...), then the mean's reciprocal — the autograd bridge's values bit for bit)
+        d_perc[i] = disc_wt * (pf - 1.0f) / qf * inv_n;
+        d_fake[i] = pf / qf * inv_n;
+        d_real[i] = (pr - 1.0f) / qr * inv_n;
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+    for (int o = 16; o > 0; o >>= 1) {
+        s_perc += __shfl_xor_sync(0xffffffffu, s_perc, o);
+        s_fake += __shfl_xor_sync(0xffffffffu, s_fake, o);
+        s_real += __shfl_xor_sync(0xffffffffu, s_real, o);
+    }
+    if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = s_perc; sh[1][threadIdx.x >> 5] = s_fake; sh[2][threadIdx.x >> 5] = s_real; }
     __syncthreads();
     if (threadIdx.x < 32) {
-        s = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0f;
+        const bool on = threadIdx.x < (blockDim.x >> 5);
+        s_perc = on ? sh[0][threadIdx.x] : 0.0f; s_fake = on ? sh[1][threadIdx.x] : 0.0f; s_real = on ? sh[2][threadIdx.x] : 0.0f;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (threadIdx.x == 0 && loss) loss[0] = s / (float)n;
+        for (int o = 16; o > 0; o >>= 1) {
+            s_perc += __shfl_xor_sync(0xffffffffu, s_perc, o);
+            s_fake += __shfl_xor_sync(0xffffffffu, s_fake, o);
+            s_real += __shfl_xor_sync(0xffffffffu, s_real, o);
+        }
+        if (threadIdx.x == 0) {
+            loss[2] = disc_wt > 0.0f ? s_perc * inv_n : 0.0f;
+            loss[4] = s_real * inv_n;
+            loss[5] = s_fake * inv_n;
+        }
     }
 }
 

@@ -905,6 +905,7 @@ int w2l_train_backward(w2l_ctx* ctx, int net, const float* d0, const float* d1, 
     cudaStream_t st = (cudaStream_t)stream;
     if (net == W2L_NET_SYNCNET && !d1) return fail(W2L_EINVAL, "null argument");
     if (dinput && !tp->input_grad) return fail(W2L_ESTATE, "the forward was not run with W2L_TRAIN_INPUT_GRAD");
+    flags &= TRAIN_WGRAD | TRAIN_ACCUMULATE | TRAIN_INPUT_GRAD | TRAIN_NO_STAT_UPDATE;   // (the fused steps' own passes are internal)
     if (net == W2L_NET_GENERATOR) flags |= TRAIN_WGRAD;
     CKR(train_backward(ctx, tp, d0, d1, flags, st));
     if (dinput) {
@@ -967,6 +968,18 @@ int w2l_comm_init(w2l_ctx* ctx, const char* id128, int rank, int world) {
     return W2L_OK;
 }
 
+// get_sync_loss (wav2lip_train.py:192-198) on the generator output of the step, and its input gradient scaled by
+// syncnet_wt (sp->dface_in); the scripts leave the frozen expert in train mode (:187-189): batch statistics, running
+// averages move
+static int sync_loss_grad(w2l_ctx* ctx, TrainPlan* sp, const float* mel, int B, float syncnet_wt, float* loss, cudaStream_t st) {
+    TrainState* ts = train_state(ctx);
+    CKR(train_forward(ctx, sp, mel, ts->g_buf, ts->a_emb, ts->v_emb, 0, st));
+    CKR(w2l_cosine_bce_loss(ctx, ts->a_emb, ts->v_emb, nullptr, B, 512, loss, st));
+    cosine_bce_bwd_kernel<<<(B + 3) / 4, 128, 0, st>>>(ts->a_emb, ts->v_emb, nullptr, syncnet_wt, ts->da, ts->dv, B, 512);
+    ctx->launches++;
+    return train_backward(ctx, sp, ts->da, ts->dv, 0, st);
+}
+
 /* one iteration of wav2lip_train.py:210-231 on the bound generator (+ frozen expert), everything on `stream` */
 int w2l_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels, const float* x, const float* mel, const float* gt, int B, int T,
                            float syncnet_wt, float lr, float* losses_dev, void* stream) {
@@ -987,13 +1000,7 @@ int w2l_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels, const float* x
     GenLossGradParams lp;
     memset(&lp, 0, sizeof(lp));
     if (sp) {
-        // get_sync_loss (:192-198); the scripts leave the frozen expert in train mode (:187-189): batch statistics, running
-        // averages move
-        CKR(train_forward(ctx, sp, mel, ts->g_buf, ts->a_emb, ts->v_emb, 0, st));
-        CKR(w2l_cosine_bce_loss(ctx, ts->a_emb, ts->v_emb, nullptr, B, 512, L + 0, st));
-        cosine_bce_bwd_kernel<<<(B + 3) / 4, 128, 0, st>>>(ts->a_emb, ts->v_emb, nullptr, syncnet_wt, ts->da, ts->dv, B, 512);
-        ctx->launches++;
-        CKR(train_backward(ctx, sp, ts->da, ts->dv, 0, st));
+        CKR(sync_loss_grad(ctx, sp, mel, B, syncnet_wt, L + 0, st));
         lp.dsync = sp->dface_in.ptr();
     }
     CKR(w2l_l1_loss(ctx, ts->g_buf, gt, numel, L + 1, st));
@@ -1009,6 +1016,173 @@ int w2l_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels, const float* x
     ctx->launches++;
     if (losses_dev) CK(cudaMemcpyAsync(losses_dev, L, 4 * 4, cudaMemcpyDeviceToDevice, st));
     CK(cudaGetLastError());
+    return W2L_OK;
+}
+
+/* one iteration of hq_wav2lip_train.py:212-256 on the bound generator, (frozen) expert and discriminator.
+ *
+ * The discriminator runs forward twice, on g (plan with input gradient) and on gt: disc(g.detach()) at :252 is the
+ * value disc(g) had at :233 (same weights — disc_optimizer.step() comes at :256 — same input, no BatchNorm or dropout),
+ * so the g tape serves two backward passes: the perceptual one (input gradient only; :246 zeroes the disc gradients it
+ * would make) and the fake term's (parameter gradients added to the real term's, no input gradient).  The two passes share
+ * the plan's gradient buffers, so they are ordered on the main stream: the perceptual pass first, then the discriminator's
+ * step (real pass, fake pass, all-reduce, Adam) forks onto its own stream and runs beside the generator's backward and
+ * Adam; the caller's stream joins it before the losses are final (and so before the next step repacks the disc slabs). */
+int w2l_hq_wav2lip_train_step(w2l_ctx* ctx, const float* indiv_mels, const float* x, const float* mel, const float* gt, int B, int T,
+                              float syncnet_wt, float disc_wt, float lr, float disc_lr, float* losses_dev, void* stream) {
+    if (!ctx || !indiv_mels || !x || !gt) return fail(W2L_EINVAL, "null argument");
+    if (B <= 0 || T <= 0) return fail(W2L_EINVAL, "bad batch B=%d T=%d", B, T);
+    if (!(syncnet_wt >= 0.0f) || !(disc_wt >= 0.0f)) return fail(W2L_EINVAL, "loss weights must be >= 0 (syncnet_wt %g, disc_wt %g)", syncnet_wt, disc_wt);
+    if (syncnet_wt > 0.0f && (!mel || T != 5)) return fail(W2L_EINVAL, "the sync loss needs mel and T == 5 (syncnet_T)");
+    DeviceGuard g(ctx->device);
+    TrainState* ts = train_state(ctx);
+    if (!ts->is_bound[W2L_NET_DISC]) return fail(W2L_ESTATE, "hq step: the discriminator is not bound (w2l_train_bind, W2L_NET_DISC)");
+    cudaStream_t st = (cudaStream_t)stream;
+    CKR(ensure_train_scratch(ctx, B, T));
+    TrainPlan *gp, *sp = nullptr, *dg, *dr;
+    CKR(get_train_plan(ctx, W2L_NET_GENERATOR, B, T, true, false, &gp));
+    if (syncnet_wt > 0.0f) CKR(get_train_plan(ctx, W2L_NET_SYNCNET, B, T, false, true, &sp));
+    CKR(get_train_plan(ctx, W2L_NET_DISC, B, T, true, true, &dg));    // on g: input gradient (perceptual) + wgrad (fake term)
+    CKR(get_train_plan(ctx, W2L_NET_DISC, B, T, true, false, &dr));   // on gt: wgrad (real term)
+    const int N = B * T;
+    float* L = ts->loss_dev;   // [0] sync, [1] l1, [2] perceptual, [3] total, [4] disc real, [5] disc fake
+    float *p_fake = ts->prob, *p_real = ts->prob + N;
+    float *d_perc = ts->dprob, *d_fake = ts->dprob + N, *d_real = ts->dprob + 2 * N;
+    CK(cudaMemsetAsync(L, 0, 6 * 4, st));
+    CKR(train_forward(ctx, gp, indiv_mels, x, ts->g_buf, nullptr, 0, st));
+    const long long numel = (long long)B * 3 * T * 9216;
+    GenLossGradParams lp;
+    memset(&lp, 0, sizeof(lp));
+    if (sp) {
+        CKR(sync_loss_grad(ctx, sp, mel, B, syncnet_wt, L + 0, st));
+        lp.dsync = sp->dface_in.ptr();
+    }
+    CKR(train_forward(ctx, dg, ts->g_buf, nullptr, p_fake, nullptr, 0, st));
+    CKR(train_forward(ctx, dr, gt, nullptr, p_real, nullptr, 0, st));
+    disc_bce_kernel<<<1, 1024, 0, st>>>(p_fake, p_real, N, disc_wt, L, d_perc, d_fake, d_real);
+    ctx->launches++;
+    if (disc_wt > 0.0f) {   // perceptual_forward (wav2lip.py:163-174) backward: dL/dg through the disc, no disc gradients
+        CKR(train_backward(ctx, dg, d_perc, nullptr, 0, st));
+        lp.ddisc = dg->dframes_in.ptr();
+    }
+    // ---- the discriminator's step (:245-256) on its own lane ----
+    cudaStream_t sd = st;
+    if (ctx->use_aux_stream) {
+        CKR(ensure_disc_stream(ts));
+        sd = ts->s_disc;
+        CK(cudaEventRecord(ts->ev_disc_fork, st));
+        CK(cudaStreamWaitEvent(sd, ts->ev_disc_fork, 0));
+    }
+    CKR(train_backward(ctx, dr, d_real, nullptr, TRAIN_WGRAD | TRAIN_ONE_STREAM, sd));
+    CKR(train_backward(ctx, dg, d_fake, nullptr, TRAIN_WGRAD | TRAIN_ACCUMULATE | TRAIN_SKIP_INPUT_GRAD | TRAIN_ONE_STREAM, sd));
+    // ---- the generator's backward and Adam (:242-243) on the caller's stream ----
+    CKR(w2l_l1_loss(ctx, ts->g_buf, gt, numel, L + 1, st));
+    // dL/dg of the L1 term in autograd's operation order — the weight (1 - syncnet_wt - disc_wt, formed in double as the
+    // script's Python floats are, rounded once) times the mean's reciprocal 1/numel, times sign(g - gt) — so that with
+    // syncnet_wt = 0 the generator's gradient equals the script's loss.backward() bit for bit
+    const float wt_l1 = (float)(1.0 - (double)syncnet_wt - (double)disc_wt);
+    lp.g = ts->g_buf; lp.gt = gt; lp.dg = ts->dg_buf; lp.l1_scale = wt_l1 * (1.0f / (float)numel); lp.B = B; lp.T = T;
+    {
+        const int blocks = (int)std::min<long long>((numel + 255) / 256, ctx->num_sms * 16);
+        gen_loss_grad_kernel<true><<<blocks, 256, 0, st>>>(lp);
+        ctx->launches++;
+    }
+    CKR(generator_backward_dp(ctx, gp, ts->dg_buf, st));
+    CKR(adam_step(ctx, W2L_NET_GENERATOR, lr, 0.5f, 0.999f, 1e-8f, 1.0f, st));   // :421-422
+    // the discriminator's bucket goes to the communication stream AFTER the generator's three, so that none of those waits
+    // for the discriminator's backward; its Adam waits for it (last_allreduce_bytes, reset by the generator's backward,
+    // ends as this step's total)
+    if (ts->world > 1 && ts->comm) {
+        CKR(all_reduce_ranges(ctx, bucket_ranges(ts, W2L_NET_DISC, {""}), sd));
+        CKR(join_comm(ctx, sd));
+    }
+    CKR(adam_step(ctx, W2L_NET_DISC, disc_lr, 0.5f, 0.999f, 1e-8f, 1.0f, sd));   // hq_wav2lip_train.py:423-424
+    if (sd != st) {
+        CK(cudaEventRecord(ts->ev_disc_join, sd));
+        CK(cudaStreamWaitEvent(st, ts->ev_disc_join, 0));
+    }
+    combine_losses_kernel<<<1, 32, 0, st>>>(L, syncnet_wt, disc_wt);
+    ctx->launches++;
+    if (losses_dev) CK(cudaMemcpyAsync(losses_dev, L, 6 * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaGetLastError());
+    return W2L_OK;
+}
+
+/* one iteration of color_syncnet_train.py:149-163 on the bound expert, everything on `stream` (the audio encoder on the
+ * auxiliary lane) */
+int w2l_syncnet_train_step(w2l_ctx* ctx, const float* mel, const float* x, const float* y, int B, float lr, float* loss_dev, void* stream) {
+    if (!ctx || !mel || !x || !y) return fail(W2L_EINVAL, "null argument");
+    if (B <= 0) return fail(W2L_EINVAL, "bad batch B=%d", B);
+    DeviceGuard g(ctx->device);
+    TrainState* ts = train_state(ctx);
+    cudaStream_t st = (cudaStream_t)stream;
+    CKR(ensure_train_scratch(ctx, B, 0));
+    TrainPlan* sp;
+    CKR(get_train_plan(ctx, W2L_NET_SYNCNET, B, 0, true, false, &sp));
+    float* L = ts->loss_dev;
+    CKR(train_forward(ctx, sp, mel, x, ts->a_emb, ts->v_emb, 0, st));
+    CKR(w2l_cosine_bce_loss(ctx, ts->a_emb, ts->v_emb, y, B, 512, L, st));
+    cosine_bce_bwd_kernel<<<(B + 3) / 4, 128, 0, st>>>(ts->a_emb, ts->v_emb, y, 1.0f, ts->da, ts->dv, B, 512);
+    ctx->launches++;
+    if (ts->world > 1 && ts->comm) {
+        // two buckets in the order the backward completes them: the face encoder (main stream), then the audio encoder
+        // (auxiliary lane, joined at the last block)
+        size_t k_face = 0;
+        for (size_t k = 0; k < sp->blocks.size(); ++k)
+            if (sp->blocks[k].lane == 0) { k_face = k; break; }
+        const std::vector<GradRange> rf = bucket_ranges(ts, W2L_NET_SYNCNET, {"face_encoder."});
+        const std::vector<GradRange> ra = bucket_ranges(ts, W2L_NET_SYNCNET, {"audio_encoder."});
+        ts->last_allreduce_bytes = 0;
+        std::function<int(size_t)> hook = [&](size_t k) -> int {
+            if (k == k_face) return all_reduce_ranges(ctx, rf, st);
+            if (k == 0) return all_reduce_ranges(ctx, ra, st);
+            return W2L_OK;
+        };
+        CKR(train_backward(ctx, sp, ts->da, ts->dv, TRAIN_WGRAD, st, &hook));
+        CKR(join_comm(ctx, st));
+    } else {
+        CKR(train_backward(ctx, sp, ts->da, ts->dv, TRAIN_WGRAD, st));
+    }
+    CKR(adam_step(ctx, W2L_NET_SYNCNET, lr, 0.9f, 0.999f, 1e-8f, 1.0f, st));   // color_syncnet_train.py:270-271
+    if (loss_dev) CK(cudaMemcpyAsync(loss_dev, L, 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaGetLastError());
+    return W2L_OK;
+}
+
+/* Adam moments and step count of named bound tensors of `net`, out of the context (direction 0) or into it (1). */
+int w2l_adam_state(w2l_ctx* ctx, int net, int direction, int n, const char* const* names, float* const* m_ptrs, float* const* v_ptrs,
+                   int64_t* step, void* stream) {
+    if (!ctx || !step || (n > 0 && (!names || !m_ptrs || !v_ptrs))) return fail(W2L_EINVAL, "null argument");
+    if (net < 0 || net > 2 || n < 0 || (direction != 0 && direction != 1)) return fail(W2L_EINVAL, "bad argument net=%d n=%d direction=%d", net, n, direction);
+    if (direction == 1 && *step < 0) return fail(W2L_EINVAL, "negative step count %lld", (long long)*step);
+    DeviceGuard g(ctx->device);
+    TrainState* ts = train_state(ctx);
+    if (!ts->is_bound[net]) return fail(W2L_ESTATE, "adam state: net %d is not bound", net);
+    cudaStream_t st = (cudaStream_t)stream;
+    CKR(ensure_adam_slot(ctx, net, st));
+    AdamSlot& a = ts->adam[net];
+    std::vector<size_t> idx((size_t)n);
+    for (int i = 0; i < n; ++i) {   // resolve every name before anything is copied
+        if (!names[i] || !m_ptrs[i] || !v_ptrs[i]) return fail(W2L_EINVAL, "null argument");
+        std::string nm = names[i];
+        if (nm.rfind("module.", 0) == 0) nm = nm.substr(7);
+        auto it = std::lower_bound(a.names.begin(), a.names.end(), nm);
+        if (it == a.names.end() || *it != nm) return fail(W2L_EINVAL, "adam state: '%s' is not a bound tensor with a gradient", nm.c_str());
+        idx[i] = (size_t)(it - a.names.begin());
+    }
+    for (int i = 0; i < n; ++i) {
+        const AdamTensor& t = a.host[idx[i]];
+        const size_t bytes = (size_t)t.n * 4;
+        if (direction == 0) {
+            CK(cudaMemcpyAsync(m_ptrs[i], t.m, bytes, cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(v_ptrs[i], t.v, bytes, cudaMemcpyDeviceToDevice, st));
+        } else {
+            CK(cudaMemcpyAsync(t.m, m_ptrs[i], bytes, cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(t.v, v_ptrs[i], bytes, cudaMemcpyDeviceToDevice, st));
+        }
+    }
+    if (direction == 0) *step = (int64_t)a.step;
+    else a.step = (long long)*step;
     return W2L_OK;
 }
 
@@ -1071,7 +1245,7 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
         }
         {
             TBlock c = b; c.dg0 = c.dg1 = 0; c.wg.on = false;
-            r = timed(b.L.name + " bwd_bn", 0, [&]() -> int { return block_backward(ctx, tp, c, false, false, st); });
+            r = timed(b.L.name + " bwd_bn", 0, [&]() -> int { return block_backward(ctx, tp, c, false, false, true, st); });
             if (r != W2L_OK) break;
         }
         if (b.dg1 > b.dg0) {
@@ -1156,7 +1330,7 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     }
     if (r == W2L_OK && dy) {
         r = launch_ingest(ctx, tp.pl.ops[tp.ingest[1]], dy, st);
-        if (r == W2L_OK) r = block_backward(ctx, &tp, tp.blocks[0], dw != nullptr, false, st);
+        if (r == W2L_OK) r = block_backward(ctx, &tp, tp.blocks[0], dw != nullptr, false, true, st);
         if (r == W2L_OK && dx) {
             const long long total = (long long)N * L.cin * H * W;
             const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);

@@ -8,6 +8,11 @@
 * `Wav2LipTrainStep`: the same iteration as ONE native call (`w2l_wav2lip_train_step`: generator forward, the frozen
   expert in train mode as the scripts leave it, both losses and their gradients, backward, bucketed gradient all-reduce
   over NCCL overlapped with the backward, multi-tensor Adam) — what bench.py --workload train times;
+* `HQWav2LipTrainStep` (`w2l_hq_wav2lip_train_step`, hq_wav2lip_train.py:212-256, with the quality discriminator and its
+  own step) and `SyncNetTrainStep` (`w2l_syncnet_train_step`, color_syncnet_train.py:149-163): the other two scripts'
+  iterations as one native call each;
+* the fused steps' Adam state as `torch.optim.Adam(...).state_dict()` gives it (`optimizer_state_dict()` /
+  `load_optimizer_state_dict()`), so checkpoints move between the reference's scripts and the fused steps;
 * `init_data_parallel`: hands every rank's context the NCCL communicator (unique id from rank 0, broadcast with
   torch.distributed).
 
@@ -26,8 +31,9 @@ class _Binding:
     """One module's tensors bound to a training context: fp32 master parameters and BatchNorm buffers by reference,
     gradients in ONE contiguous fp32 arena in state_dict order (so the all-reduce runs over three large buckets)."""
 
-    def __init__(self, module, device_index: int):
-        self.ctx = _lib.Context(device_index, _lib.PREC_BF16)
+    def __init__(self, module, device_index: int, ctx=None):
+        # (ctx: bind into another module's context — the expert and the discriminator inside a generator step)
+        self.ctx = ctx if ctx is not None else _lib.Context(device_index, _lib.PREC_BF16)
         self.device = torch.device("cuda", device_index)
         self.module = module
         self.key = None
@@ -187,8 +193,125 @@ def train_forward(module, kind, in0, in1):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# the fused native step
+# the fused native steps
 # ----------------------------------------------------------------------------------------------------------------------
+ADAM_BETAS = (0.9, 0.999)          # wav2lip_train.py:357-360, color_syncnet_train.py:270-271 (torch's default)
+HQ_ADAM_BETAS = (0.5, 0.999)       # hq_wav2lip_train.py:421-424
+
+
+def _bind_expert(b: _Binding, syncnet):
+    """The frozen expert (wav2lip_train.py:188-189) bound into the generator's context: its input gradient feeds the
+    generator's backward on the device."""
+    if syncnet is None:
+        return None
+    for q in syncnet.parameters():
+        q.requires_grad_(False)
+    return _Binding(syncnet, b.device.index, ctx=b.ctx).ensure()
+
+
+def _generator_batch(b: _Binding, x, indiv_mels, mel, gt, want_mel: bool):
+    """The generator steps' inputs, checked and made fp32 contiguous: (x, indiv_mels, mel or None, gt, B, T)."""
+    _check(b, x, indiv_mels, mel, gt)
+    x, indiv_mels, gt = _f32(x), _f32(indiv_mels), _f32(gt)
+    B, T = x.shape[0], x.shape[2] if x.dim() == 5 else 0
+    if tuple(x.shape) != (B, 6, T, 96, 96) or tuple(indiv_mels.shape) != (B, T, 1, 80, 16) or tuple(gt.shape) != (B, 3, T, 96, 96):
+        raise ValueError(f"expected x (B,6,T,96,96), indiv_mels (B,T,1,80,16), gt (B,3,T,96,96); got {tuple(x.shape)}, "
+                         f"{tuple(indiv_mels.shape)}, {tuple(gt.shape)}")
+    mel = _f32(mel) if want_mel and mel is not None else None
+    if mel is not None:
+        if tuple(mel.shape) != (B, 1, 80, 16):
+            raise ValueError(f"expected mel (B,1,80,16), got {tuple(mel.shape)}")
+    return x, indiv_mels, mel, gt, B, T
+
+
+# ---- optimizer state: torch.optim.Adam's state_dict() <-> the moments of the fused steps, mapped by parameter name ----
+def adam_param_names(module) -> list:
+    """Names of `[p for p in module.parameters() if p.requires_grad]`, the list the reference scripts hand to
+    torch.optim.Adam: entry i of its state_dict()['state'] belongs to names[i]."""
+    return [n for n, p in module.named_parameters() if p.requires_grad]
+
+
+def adam_state_to_named(sd: dict, names: list) -> dict:
+    """torch.optim.Adam(params).state_dict() (one param group over `names`) -> {'step': int, 'exp_avg': {name: t},
+    'exp_avg_sq': {name: t}, 'param_groups': [...]}.  Every state entry shares one step count (one optimizer, one
+    iteration counter); a state without entries (no step taken) has step 0."""
+    groups = sd["param_groups"]
+    if len(groups) != 1 or list(groups[0]["params"]) != list(range(len(names))):
+        raise ValueError(f"expected one Adam param group over {len(names)} parameters, got "
+                         f"{[len(g['params']) for g in groups]}")
+    steps = {float(st["step"]) for st in sd["state"].values()}
+    if len(steps) > 1:
+        raise ValueError(f"Adam state entries with different step counts {sorted(steps)}")
+    for i in sd["state"]:
+        if not 0 <= int(i) < len(names):
+            raise ValueError(f"Adam state entry {i} is outside the {len(names)} parameters")
+    step = int(steps.pop()) if steps else 0
+    return {"step": step,
+            "exp_avg": {names[int(i)]: st["exp_avg"] for i, st in sd["state"].items()},
+            "exp_avg_sq": {names[int(i)]: st["exp_avg_sq"] for i, st in sd["state"].items()},
+            "param_groups": groups}
+
+
+def adam_state_from_named(named: dict, names: list) -> dict:
+    """The inverse of adam_state_to_named: the state_dict() torch.optim.Adam would give."""
+    index = {n: i for i, n in enumerate(names)}
+    unknown = set(named["exp_avg"]) - set(index)
+    if unknown:
+        raise ValueError(f"moments of unknown parameters: {sorted(unknown)[:4]}")
+    state = {}
+    for n in sorted(named["exp_avg"], key=index.get):
+        state[index[n]] = {"step": torch.tensor(float(named["step"]), dtype=torch.float32),
+                           "exp_avg": named["exp_avg"][n], "exp_avg_sq": named["exp_avg_sq"][n]}
+    return {"state": state, "param_groups": named["param_groups"]}
+
+
+def _adam_call(b: _Binding, net: int, direction: int, names: list, m: list, v: list, step: int) -> int:
+    k = len(names)
+    s = C.c_int64(step)
+    _lib.check(b.ctx.lib.w2l_adam_state(b.ctx.h, net, direction, k, (C.c_char_p * k)(*[n.encode() for n in names]),
+                                        (C.c_void_p * k)(*[t.data_ptr() for t in m]), (C.c_void_p * k)(*[t.data_ptr() for t in v]),
+                                        C.byref(s), _stream(b)))
+    return int(s.value)
+
+
+def _export_adam(b: _Binding, module, lr: float, betas) -> dict:
+    b.ensure()
+    names = adam_param_names(module)
+    params = dict(module.named_parameters())
+    m = [torch.empty_like(params[n]) for n in names]
+    v = [torch.empty_like(params[n]) for n in names]
+    step = _adam_call(b, module.NET, 0, names, m, v, 0)
+    groups = torch.optim.Adam([params[n] for n in names], lr=lr, betas=betas).state_dict()["param_groups"]
+    named = {"step": step, "exp_avg": dict(zip(names, m)) if step else {}, "exp_avg_sq": dict(zip(names, v)) if step else {},
+             "param_groups": groups}
+    return adam_state_from_named(named, names)
+
+
+def _import_adam(b: _Binding, module, sd: dict, betas) -> float:
+    """Loads sd into the context's Adam of `module`; returns the saved learning rate."""
+    b.ensure()
+    names = adam_param_names(module)
+    named = adam_state_to_named(sd, names)
+    group = named["param_groups"][0]
+    if tuple(group["betas"]) != tuple(betas):
+        raise ValueError(f"optimizer state with betas {tuple(group['betas'])}, this step runs Adam with {tuple(betas)}")
+    params = dict(module.named_parameters())
+    if named["step"] and set(named["exp_avg"]) != set(names):
+        raise ValueError(f"optimizer state has moments for {len(named['exp_avg'])} of {len(names)} parameters")
+
+    def moment(which, n):
+        t = named[which].get(n)
+        if t is None:
+            return torch.zeros_like(params[n])
+        if t.numel() != params[n].numel():
+            raise ValueError(f"{which} of {n}: {tuple(t.shape)}, parameter {tuple(params[n].shape)}")
+        return t.detach().to(device=b.device, dtype=torch.float32).reshape(params[n].shape).contiguous()
+    m = [moment("exp_avg", n) for n in names]
+    v = [moment("exp_avg_sq", n) for n in names]
+    _adam_call(b, module.NET, 1, names, m, v, named["step"])
+    return float(group["lr"])
+
+
 class Wav2LipTrainStep:
     """wav2lip_train.py:210-231 as one native call per iteration.
 
@@ -207,50 +330,137 @@ class Wav2LipTrainStep:
             raise _lib.W2LError("move the model to a CUDA device first: wav2lip_b200 has no CPU path")
         self.b = binding_of(model, p)
         self.losses = torch.zeros(4, device=p.device, dtype=torch.float32)
-        if syncnet is not None:
-            for q in syncnet.parameters():
-                q.requires_grad_(False)      # wav2lip_train.py:188-189
-            self._bind_expert()
-
-    def _bind_expert(self):
-        # the expert shares the generator's context (its input gradient feeds the generator's backward on the device)
-        s, b = self.syncnet, self.b
-        names, values, grads, numels, self._nbt = [], [], [], [], []
-        for n, t in s.state_dict(keep_vars=True).items():
-            if not t.dtype.is_floating_point:
-                if n.endswith("num_batches_tracked"):
-                    self._nbt.append(t)
-                continue
-            if not t.is_cuda or t.device != b.device:
-                raise _lib.W2LError(f"syncnet tensor {n} is on {t.device}, expected {b.device}")
-            names.append(n.encode()); values.append(t.data_ptr()); grads.append(None); numels.append(t.numel())
-        k = len(names)
-        _lib.check(b.ctx.lib.w2l_train_bind(b.ctx.h, _lib.NET_SYNCNET, k, (C.c_char_p * k)(*names), (C.c_void_p * k)(*values),
-                                            (C.c_void_p * k)(*grads), (C.c_int64 * k)(*numels)))
+        self.eb = _bind_expert(self.b, syncnet)
 
     def __call__(self, x, indiv_mels, mel, gt):
         b = self.b.ensure()
-        _check(b, x, indiv_mels, mel, gt)
-        x, indiv_mels, gt = _f32(x), _f32(indiv_mels), _f32(gt)
-        B, T = x.shape[0], x.shape[2]
-        if tuple(x.shape) != (B, 6, T, 96, 96) or tuple(indiv_mels.shape) != (B, T, 1, 80, 16) or tuple(gt.shape) != (B, 3, T, 96, 96):
-            raise ValueError(f"expected x (B,6,T,96,96), indiv_mels (B,T,1,80,16), gt (B,3,T,96,96); got {tuple(x.shape)}, "
-                             f"{tuple(indiv_mels.shape)}, {tuple(gt.shape)}")
         wt = self.syncnet_wt if self.syncnet is not None else 0.0
-        m = _f32(mel) if wt > 0 else None
+        x, indiv_mels, m, gt, B, T = _generator_batch(b, x, indiv_mels, mel, gt, wt > 0)
+        if self.eb is not None:
+            self.eb.ensure()
         _lib.check(b.ctx.lib.w2l_wav2lip_train_step(b.ctx.h, _P(indiv_mels), _P(x), _P(m), _P(gt), B, T, wt, self.lr,
                                                     _P(self.losses), _stream(b)))
         b.bump_batches_tracked()
-        if wt > 0 and self._nbt:
-            torch._foreach_add_(self._nbt, 1)
+        if wt > 0:
+            self.eb.bump_batches_tracked()
         self.model.mark_weights_dirty()
         return self.losses
+
+    def optimizer_state_dict(self) -> dict:
+        """`optimizer.state_dict()` of wav2lip_train.py's `optim.Adam([p for p in model.parameters() if p.requires_grad],
+        lr)` after the steps run so far."""
+        return _export_adam(self.b, self.model, self.lr, ADAM_BETAS)
+
+    def load_optimizer_state_dict(self, sd: dict) -> None:
+        """`optimizer.load_state_dict(sd)` (load_checkpoint(..., reset_optimizer=False)); takes the saved lr, as torch does."""
+        self.lr = _import_adam(self.b, self.model, sd, ADAM_BETAS)
 
     def last_output(self, B: int, T: int) -> torch.Tensor:
         """g of the last step, (B,3,T,96,96) fp32 (a copy)."""
         out = torch.empty((B, 3, T, 96, 96), device=self.b.device, dtype=torch.float32)
         _lib.check(self.b.ctx.lib.w2l_train_last_output(self.b.ctx.h, _P(out), out.numel(), _stream(self.b)))
         return out
+
+
+class HQWav2LipTrainStep:
+    """hq_wav2lip_train.py:212-256 as one native call per iteration.
+
+        step = HQWav2LipTrainStep(model, disc, syncnet, lr=1e-4, disc_lr=1e-4, syncnet_wt=0.0, disc_wt=0.07)
+        losses = step(x, indiv_mels, mel, gt)   # device tensor [sync, l1, perceptual, loss, disc_real, disc_fake]
+
+    The generator, the frozen expert and the discriminator share one training context; both networks' parameters are
+    updated in place by their Adam (betas 0.5, 0.999).  `syncnet_wt` / `disc_wt` may be changed between calls (the script
+    switches the sync loss on with hparams.set_hparam('syncnet_wt', ...)).  With `init_data_parallel(step)` both networks'
+    gradients are averaged over the ranks inside the step."""
+
+    def __init__(self, model, disc, syncnet=None, lr: float = 1e-4, disc_lr: float = 1e-4, syncnet_wt: float = 0.0,
+                 disc_wt: float = 0.07):
+        self.model, self.disc, self.syncnet = model, disc, syncnet
+        self.lr, self.disc_lr, self.syncnet_wt, self.disc_wt = float(lr), float(disc_lr), float(syncnet_wt), float(disc_wt)
+        p = next(model.parameters())
+        if not p.is_cuda:
+            raise _lib.W2LError("move the model to a CUDA device first: wav2lip_b200 has no CPU path")
+        self.b = binding_of(model, p)
+        self.db = _Binding(disc, self.b.device.index, ctx=self.b.ctx).ensure()
+        self.eb = _bind_expert(self.b, syncnet)
+        self.losses = torch.zeros(6, device=p.device, dtype=torch.float32)
+        self._shape = None
+
+    def __call__(self, x, indiv_mels, mel, gt):
+        b = self.b.ensure()
+        self.db.ensure()
+        wt = self.syncnet_wt if self.syncnet is not None else 0.0
+        x, indiv_mels, mel, gt, B, T = _generator_batch(b, x, indiv_mels, mel, gt, wt > 0)
+        if self.eb is not None:
+            self.eb.ensure()
+        _lib.check(b.ctx.lib.w2l_hq_wav2lip_train_step(b.ctx.h, _P(indiv_mels), _P(x), _P(mel), _P(gt), B, T,
+                                                       wt, self.disc_wt, self.lr, self.disc_lr, _P(self.losses), _stream(b)))
+        b.bump_batches_tracked()
+        if wt > 0:
+            self.eb.bump_batches_tracked()
+        self.model.mark_weights_dirty()
+        self.disc.mark_weights_dirty()
+        self._shape = (B, T)
+        return self.losses
+
+    def last_output(self, B: int = None, T: int = None) -> torch.Tensor:
+        """g of the last step, (B,3,T,96,96) fp32 (a copy)."""
+        B, T = (B, T) if B is not None else self._shape
+        out = torch.empty((B, 3, T, 96, 96), device=self.b.device, dtype=torch.float32)
+        _lib.check(self.b.ctx.lib.w2l_train_last_output(self.b.ctx.h, _P(out), out.numel(), _stream(self.b)))
+        return out
+
+    def optimizer_state_dict(self) -> dict:
+        """`optimizer.state_dict()` of the generator's Adam (hq_wav2lip_train.py:421-422)."""
+        return _export_adam(self.b, self.model, self.lr, HQ_ADAM_BETAS)
+
+    def load_optimizer_state_dict(self, sd: dict) -> None:
+        self.lr = _import_adam(self.b, self.model, sd, HQ_ADAM_BETAS)
+
+    def disc_optimizer_state_dict(self) -> dict:
+        """`disc_optimizer.state_dict()` (hq_wav2lip_train.py:423-424), saved in its own checkpoint file (:280-282)."""
+        return _export_adam(self.db, self.disc, self.disc_lr, HQ_ADAM_BETAS)
+
+    def load_disc_optimizer_state_dict(self, sd: dict) -> None:
+        self.disc_lr = _import_adam(self.db, self.disc, sd, HQ_ADAM_BETAS)
+
+
+class SyncNetTrainStep:
+    """color_syncnet_train.py:149-163 as one native call per iteration.
+
+        step = SyncNetTrainStep(model, lr=1e-4)
+        loss = step(x, mel, y)      # x (B,15,48,96), mel (B,1,80,16), y (B,1) in {0,1} (SyncNetBatches); device tensor [loss]
+
+    Adam with torch's default betas (:270-271) updates the parameters in place; with `init_data_parallel(step)` the
+    gradients are averaged over the ranks inside the step."""
+
+    def __init__(self, model, lr: float = 1e-4):
+        self.model, self.lr = model, float(lr)
+        p = next(model.parameters())
+        if not p.is_cuda:
+            raise _lib.W2LError("move the model to a CUDA device first: wav2lip_b200 has no CPU path")
+        self.b = binding_of(model, p)
+        self.loss = torch.zeros(1, device=p.device, dtype=torch.float32)
+
+    def __call__(self, x, mel, y):
+        b = self.b.ensure()
+        _check(b, x, mel, y)
+        x, mel, y = _f32(x), _f32(mel), _f32(y)
+        B = x.shape[0]
+        if tuple(x.shape) != (B, 15, 48, 96) or tuple(mel.shape) != (B, 1, 80, 16) or tuple(y.shape) != (B, 1):
+            raise ValueError(f"expected x (B,15,48,96), mel (B,1,80,16), y (B,1); got {tuple(x.shape)}, {tuple(mel.shape)}, "
+                             f"{tuple(y.shape)}")
+        _lib.check(b.ctx.lib.w2l_syncnet_train_step(b.ctx.h, _P(mel), _P(x), _P(y), B, self.lr, _P(self.loss), _stream(b)))
+        b.bump_batches_tracked()
+        self.model.mark_weights_dirty()
+        return self.loss
+
+    def optimizer_state_dict(self) -> dict:
+        """`optimizer.state_dict()` of color_syncnet_train.py's Adam."""
+        return _export_adam(self.b, self.model, self.lr, ADAM_BETAS)
+
+    def load_optimizer_state_dict(self, sd: dict) -> None:
+        self.lr = _import_adam(self.b, self.model, sd, ADAM_BETAS)
 
 
 def init_data_parallel(step_or_binding) -> int:
