@@ -93,7 +93,32 @@ def test_block_matches_oracle(case):
     assert err <= REL * ref.abs().max().item(), f"max|err| {err:.4g} vs max|ref| {ref.abs().max().item():.4g}"
 
 
+# Block descriptions the C ABI's single-block entries must refuse before they allocate or launch anything:
+# (what is wrong, kind, cin, cout, kh, kw, sh, sw, ph, pw, residual), applied to a (1, cin, 8, 8) input
+BAD_LAYERS = [
+    ("stride 0", 0, 64, 64, 3, 3, 0, 1, 1, 1, 0),
+    ("8x8 kernel", 0, 64, 64, 8, 8, 1, 1, 3, 3, 0),
+    ("residual with cin != cout", 0, 32, 64, 3, 3, 1, 1, 1, 1, 1),
+]
+
+
+def bad_layer_calls():
+    """(what, LayerInfo, tensors) per BAD_LAYERS row; the tensors are large enough for any shape the row implies."""
+    from wav2lip_b200 import _lib
+    for what, kind, cin, cout, kh, kw, sh, sw, ph, pw, res in BAD_LAYERS:
+        li = _lib.LayerInfo()
+        li.name = b"block"
+        li.kind, li.cin, li.cout, li.kh, li.kw, li.sh, li.sw, li.ph, li.pw, li.out_pad, li.residual = (
+            kind, cin, cout, kh, kw, sh, sw, ph, pw, 0, res)
+        t = {"x": torch.zeros(1, cin, 8, 8, device="cuda"), "w": torch.zeros(cout, cin, kh, kw, device="cuda"),
+             "y": torch.zeros(1, cout, 16, 16, device="cuda")}
+        t.update({k: torch.ones(cout, device="cuda") for k in ("b", "gamma", "beta", "mean", "var")})
+        yield what, li, t
+
+
 def test_block_rejects_bad_arguments():
+    import ctypes as C
+
     from wav2lip_b200 import _lib
     from wav2lip_b200.models.conv import Conv2d
     m = Conv2d(64, 64, 3, 1, 1).eval()  # parameters on the CPU
@@ -105,3 +130,13 @@ def test_block_rejects_bad_arguments():
     m = Conv2d(64, 64, 3, 1, 1).cuda()   # train mode: batch-stat BN is not built
     with pytest.raises(NotImplementedError):
         m(torch.zeros(1, 64, 8, 8, device="cuda"))
+    ctx = _lib.Context(0, _lib.PREC_F16)
+    P = lambda a: C.c_void_p(a.data_ptr())
+    for what, li, t in bad_layer_calls():
+        torch.cuda.synchronize()
+        n0 = ctx.launch_count()
+        with pytest.raises(_lib.W2LError):
+            _lib.check(ctx.lib.w2l_conv_block_forward(ctx.h, C.byref(li), P(t["x"]), 1, 8, 8, P(t["w"]), P(t["b"]),
+                                                      P(t["gamma"]), P(t["beta"]), P(t["mean"]), P(t["var"]), P(t["y"]),
+                                                      None))
+        assert ctx.launch_count() == n0, what

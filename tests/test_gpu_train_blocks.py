@@ -172,3 +172,19 @@ def test_block_train_forward_backward(case, ctx):
     bad = {k: v for k, v in errs.items() if not (v <= REL)}
     bad.update({"loose_" + k: v for k, v in loose.items() if not (v <= LOOSE)})
     assert not bad, ({k: float(f"{v:.3g}") for k, v in errs.items()}, {k: float(f"{v:.3g}") for k, v in loose.items()})
+
+
+def test_block_train_rejects_bad_arguments(ctx):
+    """The block descriptions w2l_conv_block_forward refuses, refused by the training entry too, with nothing launched."""
+    from wav2lip_b200 import _lib
+    from test_gpu_blocks import bad_layer_calls
+    P = lambda a: C.c_void_p(a.data_ptr())
+    for what, li, t in bad_layer_calls():
+        dx, dw, grads = torch.empty_like(t["x"]), torch.empty_like(t["w"]), [torch.empty_like(t["b"]) for _ in range(3)]
+        torch.cuda.synchronize()
+        n0 = ctx.launch_count()
+        with pytest.raises(_lib.W2LError):
+            _lib.check(ctx.lib.w2l_conv_block_train(ctx.h, C.byref(li), P(t["x"]), 1, 8, 8, P(t["w"]), P(t["b"]), P(t["gamma"]),
+                                                    P(t["beta"]), P(t["mean"]), P(t["var"]), P(t["y"]), P(t["y"]), P(dx),
+                                                    P(dw), *map(P, grads), None))
+        assert ctx.launch_count() == n0, what

@@ -27,22 +27,74 @@ static int tmp_act(w2l_ctx* ctx, Plan* pl, TmpPool* tp, Act* a, int N, int H, in
     return W2L_OK;
 }
 
-static void add_ingest(Plan* pl, const char* name, int src_id, const Act& dst, int B, int C, long long sB, long long sC,
-                       long long sT, int y_off, int Wsrc) {
+// How the ingest kernel reads one fp32 caller tensor (IngestParams): destination image n = t*B + b, channel c, row y
+// comes from src + b*sB + t*sT + c*sC + (y + y_off)*Wsrc;  cgrp > 0: c*sC becomes (c / cgrp)*sG + (c % cgrp)*sC
+struct IngestSpec {
+    int src_id;          // which caller tensor: 0 = mel / frames, 1 = face
+    int B, C;
+    long long sB, sC, sT;
+    int y_off, Wsrc;
+    int cgrp = 0;
+    long long sG = 0;
+};
+
+// The caller tensors of each network, for its inference and its training plans.
+// Generator: mel (B,T,1,80,16) and face (B,6,T,96,96); T == 0: (B,1,80,16) and (B,6,96,96)
+static void generator_inputs(int B, int T, IngestSpec* mel, IngestSpec* face) {
+    if (T > 0) {
+        *mel = IngestSpec{0, B, 1, (long long)T * 1280, 1280, 1280, 0, 16};
+        *face = IngestSpec{1, B, 6, (long long)6 * T * 9216, (long long)T * 9216, 9216, 0, 96};
+    } else {
+        *mel = IngestSpec{0, B, 1, 1280, 1280, 0, 0, 16};
+        *face = IngestSpec{1, B, 6, 6 * 9216, 9216, 0, 0, 96};
+    }
+}
+
+// SyncNet: mel (B,1,80,16) and the face window (B,15,48,96); T > 0: generated / ground-truth frames (B,3,T,96,96) instead,
+// lower half, the T frames stacked on channels (c' = 3 t + c) — wav2lip_train.py:193-194 as addressing
+static void syncnet_inputs(int B, int T, IngestSpec* mel, IngestSpec* face) {
+    *mel = IngestSpec{0, B, 1, 1280, 1280, 0, 0, 16};
+    if (T > 0) *face = IngestSpec{1, B, 3 * T, (long long)3 * T * 9216, (long long)T * 9216, 0, 48, 96, 3, 9216};
+    else *face = IngestSpec{1, B, 15, 15 * 4608, 4608, 0, 0, 96};
+}
+
+// Discriminator: frames (B,3,T,96,96), t-major flatten + rows 48..95   (wav2lip.py:155-161)
+static IngestSpec disc_input(int B, int T) { return IngestSpec{0, B, 3, (long long)3 * T * 9216, (long long)T * 9216, 9216, 48, 96}; }
+
+static void add_ingest(Plan* pl, const char* name, const IngestSpec& s, const Act& dst) {
     Op op;
     op.type = OP_INGEST;
     op.name = name;
-    op.ingest_src = src_id;
+    op.ingest_src = s.src_id;
     IngestParams& ip = op.ip;
     ip.src = nullptr; ip.dst = dst.base;
-    ip.N = dst.N; ip.B = B; ip.C = C; ip.H = dst.H; ip.W = dst.W;
+    ip.N = dst.N; ip.B = s.B; ip.C = s.C; ip.H = dst.H; ip.W = dst.W;
     ip.Cpad = dst.lo_off > 0 ? dst.lo_off : dst.Cs;  // logical (padded) channels; Cs is the pixel pitch
     ip.Cpix = dst.Cs;
     ip.Wp = dst.pitch(); ip.x_off = dst.x_off;
     ip.lo_off = dst.lo_off;
-    ip.sB = sB; ip.sC = sC; ip.sT = sT; ip.y_off = y_off; ip.Wsrc = Wsrc;
-    ip.cgrp = 0; ip.sG = 0;
+    ip.sB = s.sB; ip.sC = s.sC; ip.sT = s.sT; ip.y_off = s.y_off; ip.Wsrc = s.Wsrc;
+    ip.cgrp = s.cgrp; ip.sG = s.sG;
     pl->ops.push_back(op);
+}
+
+static int launch_ingest(w2l_ctx* ctx, const Op& op, const void* src, cudaStream_t st) {
+    IngestParams ip = op.ip;
+    ip.src = (const float*)src;
+    const long long total = (long long)ip.N * ip.H * ip.W;
+    const bool vec4 = ip.lo_off == 0 && ((ip.W | ip.Wsrc) & 3) == 0 && ((ip.sB | ip.sC | ip.sT | ip.sG) & 3) == 0 &&
+                      (((uintptr_t)ip.src) & 15) == 0;
+    if (vec4) {
+        const int blocks = (int)std::min<long long>((total / 4 + 255) / 256, ctx->num_sms * 16);
+        if (ctx->bf16) ingest4_kernel<true><<<blocks, 256, 0, st>>>(ip);
+        else ingest4_kernel<false><<<blocks, 256, 0, st>>>(ip);
+    } else {
+        const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
+        if (ctx->bf16) ingest_kernel<true><<<blocks, 256, 0, st>>>(ip);
+        else ingest_kernel<false><<<blocks, 256, 0, st>>>(ip);
+    }
+    ctx->launches++;
+    return W2L_OK;
 }
 
 // a straight chain of blocks (encoders): ping-pong temporaries, optional final destination
@@ -74,19 +126,13 @@ static int build_generator_plan(w2l_ctx* ctx, Plan* pl) {
     const NetW& nw = ctx->nets[W2L_NET_GENERATOR];
     CKR(plan_input_act(pl, &faceIn, N, 96, 96, 6, nw.layers[g.face_enc[0][0]], g.layers[g.face_enc[0][0]]));
     CKR(plan_input_act(pl, &melIn, N, 80, 16, 1, nw.layers[g.audio_enc[0]], g.layers[g.audio_enc[0]]));
-    if (T > 0) {
-        add_ingest(pl, "ingest.mel", 0, melIn, B, 1, (long long)T * 1280, 1280, 1280, 0, 16);
-        add_ingest(pl, "ingest.face", 1, faceIn, B, 6, (long long)6 * T * 9216, (long long)T * 9216, 9216, 0, 96);
-    } else {
-        add_ingest(pl, "ingest.mel", 0, melIn, N, 1, 1280, 1280, 0, 0, 16);
-        add_ingest(pl, "ingest.face", 1, faceIn, N, 6, 6 * 9216, 9216, 0, 0, 96);
-    }
+    IngestSpec mel, face;
+    generator_inputs(B, T, &mel, &face);
+    add_ingest(pl, "ingest.mel", mel, melIn);
+    add_ingest(pl, "ingest.face", face, faceIn);
     // skip-concat buffers D[k]: [decoder output | encoder feature] at resolution hw[k]   (wav2lip.py:108)
-    const int hw[7] = {1, 3, 6, 12, 24, 48, 96};
-    const int dec_c[7] = {512, 512, 512, 384, 256, 128, 64};
-    const int skip_c[7] = {512, 512, 256, 128, 64, 32, 16};
     Act D[7];
-    for (int k = 0; k < 7; ++k) CKR(plan_act(pl, &D[k], N, hw[k], hw[k], dec_c[k] + skip_c[k]));
+    for (int k = 0; k < 7; ++k) CKR(plan_act(pl, &D[k], N, g.hw[k], g.hw[k], g.dec_c[k] + g.skip_c[k]));
 
     // audio encoder -> (N,1,1,512)
     Act AE;
@@ -103,7 +149,7 @@ static int build_generator_plan(w2l_ctx* ctx, Plan* pl) {
     TmpPool tpe;
     Act x = faceIn;
     for (int i = 0; i < 7; ++i) {
-        Act dst = D[6 - i].slice(dec_c[6 - i], skip_c[6 - i]);
+        Act dst = D[6 - i].slice(g.dec_c[6 - i], g.skip_c[6 - i]);
         CKR(emit_chain(ctx, pl, W2L_NET_GENERATOR, g.layers, g.face_enc[i], x, &tpe, &dst, &x));
         if (i == 0 && nw.layers[g.face_enc[1][0]].ph[0].fold) {
             // The 16->32 stride-2 block gathers every other pixel of a 16-channel slice of D[6]: 32-byte TMA rows, the
@@ -133,7 +179,7 @@ static int build_generator_plan(w2l_ctx* ctx, Plan* pl) {
     x = AE;
     const size_t dec_first = pl->ops.size();
     for (int k = 0; k < 7; ++k) {
-        Act dst = D[k].slice(0, dec_c[k]);
+        Act dst = D[k].slice(0, g.dec_c[k]);
         CKR(emit_chain(ctx, pl, W2L_NET_GENERATOR, g.layers, g.face_dec[k], x, &tpd, &dst, nullptr));
         x = D[k];
     }
@@ -155,16 +201,10 @@ static int build_syncnet_plan(w2l_ctx* ctx, Plan* pl) {
     CKR(plan_input_act(pl, &melIn, N, 80, 16, 1, nw.layers[s.audio_enc[0]], s.layers[s.audio_enc[0]]));
     CKR(plan_act(pl, &fe, N, 1, 1, 512, true));
     CKR(plan_act(pl, &ae, N, 1, 1, 512, true));
-    add_ingest(pl, "ingest.mel", 0, melIn, N, 1, 1280, 1280, 0, 0, 16);
-    if (pl->T > 0) {
-        // face input = generated / ground-truth frames (B,3,T,96,96): lower half, the T frames stacked on channels
-        // (c' = 3 t + c) — wav2lip_train.py:193-194 as addressing
-        const int T = pl->T;
-        add_ingest(pl, "ingest.frames", 1, faceIn, N, 3 * T, (long long)3 * T * 9216, (long long)T * 9216, 0, 48, 96);
-        pl->ops.back().ip.cgrp = 3; pl->ops.back().ip.sG = 9216;
-    } else {
-        add_ingest(pl, "ingest.face", 1, faceIn, N, 15, 15 * 4608, 4608, 0, 0, 96);
-    }
+    IngestSpec mel, face;
+    syncnet_inputs(N, pl->T, &mel, &face);
+    add_ingest(pl, "ingest.mel", mel, melIn);
+    add_ingest(pl, pl->T > 0 ? "ingest.frames" : "ingest.face", face, faceIn);
     TmpPool tpf, tpa;
     // the two encoders are independent until the embeddings: the audio one (short launches, issued first) runs on the
     // side stream while the face encoder runs on the main one
@@ -192,8 +232,7 @@ static int build_disc_plan(w2l_ctx* ctx, Plan* pl) {
     Act in, feat;
     CKR(plan_input_act(pl, &in, N, 48, 96, 3, ctx->nets[W2L_NET_DISC].layers[0], d.layers[0]));
     CKR(plan_act(pl, &feat, N, 1, 1, 512));
-    // (B,3,T,96,96): t-major flatten + rows 48..95   (wav2lip.py:155-161)
-    add_ingest(pl, "ingest.frames", 0, in, B, 3, (long long)3 * T * 9216, (long long)T * 9216, 9216, 48, 96);
+    add_ingest(pl, "ingest.frames", disc_input(B, T), in);
     std::vector<int> idx;
     for (size_t i = 0; i < d.layers.size(); ++i) idx.push_back((int)i);
     TmpPool tp;
@@ -228,7 +267,7 @@ static int build_s3fd_plan(w2l_ctx* ctx, Plan* pl) {
     if (H < 32 || W < 32) return fail(W2L_EINVAL, "S3FD needs an image of at least 32 x 32 (five 2x2 pools)");
     Act x;
     CKR(plan_input_act(pl, &x, N, H, W, 3, nw.layers[0], sp.layers[0]));
-    add_ingest(pl, "ingest.img", 0, x, N, 3, (long long)3 * H * W, (long long)H * W, 0, 0, W);
+    add_ingest(pl, "ingest.img", IngestSpec{0, N, 3, (long long)3 * H * W, (long long)H * W, 0, 0, W}, x);
     auto conv = [&](int li, const Act& in, Act* out, bool f32 = false) -> int {
         const Layer& L = sp.layers[li];
         int Ho, Wo;
@@ -401,21 +440,7 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
                     ctx->launches++;
                     break;
                 }
-                IngestParams ip = op.ip;
-                ip.src = (const float*)(op.ingest_src == 0 ? in0 : in1);
-                const long long total = (long long)ip.N * ip.H * ip.W;
-                const bool vec4 = ip.lo_off == 0 && ((ip.W | ip.Wsrc) & 3) == 0 && ((ip.sB | ip.sC | ip.sT | ip.sG) & 3) == 0 &&
-                                  (((uintptr_t)ip.src) & 15) == 0;
-                if (vec4) {
-                    const int blocks = (int)std::min<long long>((total / 4 + 255) / 256, ctx->num_sms * 16);
-                    if (ctx->bf16) ingest4_kernel<true><<<blocks, 256, 0, st>>>(ip);
-                    else ingest4_kernel<false><<<blocks, 256, 0, st>>>(ip);
-                } else {
-                    const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-                    if (ctx->bf16) ingest_kernel<true><<<blocks, 256, 0, st>>>(ip);
-                    else ingest_kernel<false><<<blocks, 256, 0, st>>>(ip);
-                }
-                ctx->launches++;
+                CKR(launch_ingest(ctx, op, op.ingest_src == 0 ? in0 : in1, st));
                 break;
             }
             case OP_CONV: {

@@ -55,10 +55,7 @@ struct TrainPlan {
     int net = 0, B = 0, T = 0, N = 0;
     Plan pl;                       // op storage + allocations
     NetW wf, wd;                   // forward / dgrad weight slabs (16-bit), repacked every step
-    std::vector<PackParams> pack_jobs;
-    std::vector<PackFoldParams> pack_fold_jobs;
-    std::vector<FoldJob> fold_jobs;
-    bool allow_fold = false;   // the context's own switch (the builder turns them off around itself)
+    RepackLog repack;              // ... by these launches
     PackParams* pack_dev = nullptr; int *pack_blk_job = nullptr, *pack_blk_first = nullptr; int pack_blocks = 0;   // one-launch repack
     std::vector<TBlock> blocks;    // forward order
     std::vector<size_t> ingest;    // indices of the ingest ops
@@ -191,13 +188,13 @@ static Layer dgrad_layer(const Layer& L, int Hin, int Win, int Ho, int Wo, bool 
 }
 
 // Pack the dgrad weights of block L from the master tensor W (fp32, the reference's layout).
-static int load_dgrad_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const Layer& Ld, const float* W, cudaStream_t st) {
+static int load_dgrad_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const Layer& Ld, const float* W, RepackLog* log, cudaStream_t st) {
     if (L.kind == W2L_BLOCK_CONVT_BN_RELU)     // (Cin_t, Cout_t, kh, kw) == conv layout (out, in, kh, kw): plain pack
-        return load_layer(ctx, lw, Ld, W, nullptr, nullptr, nullptr, nullptr, nullptr, false, false, st);
+        return load_layer(ctx, lw, Ld, W, nullptr, nullptr, nullptr, nullptr, nullptr, false, false, log, st);
     if (Ld.kind == W2L_BLOCK_CONVT_BN_RELU) {  // (Cout, Cin, kh, kw) == transposed-conv layout (in, out, kh, kw): phase packs
         Layer t = Ld;
         t.cout = L.cin;                        // real channel count of the source tensor (cout_pad rounds up)
-        return load_layer(ctx, lw, t, W, nullptr, nullptr, nullptr, nullptr, nullptr, false, false, st);
+        return load_layer(ctx, lw, t, W, nullptr, nullptr, nullptr, nullptr, nullptr, false, false, log, st);
     }
     // stride 1: dst[tap][ci][co] = W[co][ci][r][s], tap (r,s) reads dz at (y + ph - r, x + pw - s)
     // (Ld.cout may have been widened to a multiple of 128 — see dgrad_layer — the extra rows are zero and never stored)
@@ -206,7 +203,7 @@ static int load_dgrad_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const Laye
     PackedW pw;
     for (int r = 0; r < L.kh; ++r)
         for (int s = 0; s < L.kw; ++s) { rs.push_back({r, s}); pw.dy.push_back((signed char)(L.ph - r)); pw.dx.push_back((signed char)(L.pw - s)); }
-    CKR(pack_taps(ctx, &pw, W, L.cin, L.cout, L.kh, L.kw, true, rs, Ld.cout, st));
+    CKR(pack_taps(ctx, &pw, W, L.cin, L.cout, L.kh, L.kw, true, rs, Ld.cout, log, st));
     lw->ph.push_back(pw);
     const int n_pad = Ld.cout;
     void* sc = nullptr; void* sh = nullptr;
@@ -322,13 +319,13 @@ static int make_wgrad_op(w2l_ctx* ctx, TrainPlan* tp, TBlock* b, size_t* ws_need
     return W2L_OK;
 }
 
-static int launch_wgrad(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool accumulate, cudaStream_t st) {
+static int launch_wgrad(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool accumulate, cudaStream_t st, bool pdl = true) {
     WgKernelEntry* e = nullptr;
     for (auto& k : g_wg_kernels) if (k.BN == b.wg.BN) e = &k;
     if (!e) return fail(W2L_EINVAL, "no wgrad kernel for BN=%d", b.wg.BN);
     CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, kWgSmemMax + 2048));
     b.wg.wp.ws = tp->wg_ws[b.lane];
-    CK(launch_k(e->fn, b.wg.grid, kWgThreads, (size_t)b.wg.smem, st, b.wg.wp, ctx->use_pdl));
+    CK(launch_k(e->fn, b.wg.grid, kWgThreads, (size_t)b.wg.smem, st, b.wg.wp, pdl && ctx->use_pdl));
     WgradReduceParams rp = b.wg.rp;
     rp.ws = tp->wg_ws[b.lane]; rp.out = b.gW; rp.accumulate = accumulate ? 1 : 0;
     const int n_tiles64 = (rp.Cn + 63) / 64;
@@ -340,17 +337,20 @@ static int launch_wgrad(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool accumulate,
 // dense 16-bit activation owned by the plan
 static int tp_act(TrainPlan* tp, Act* a, int N, int H, int W, int C) { return plan_act(&tp->pl, a, N, H, W, C); }
 
-// First blocks (fed by a caller tensor): the forward conv may read a second, K-folded copy of the input (the inference
-// plan's first-layer layout, 10-20x faster on the 7x7 / 6-channel layer) written by one more ingest launch; the backward
-// (wgrad) reads the plain NHWC copy.
-struct FoldIn { bool on = false; int src_id = 0, B = 0, C = 0; long long sB = 0, sC = 0, sT = 0; int y_off = 0, Wsrc = 0, cgrp = 0; long long sG = 0; };
+static void add_train_ingest(TrainPlan* tp, const char* name, const IngestSpec& s, const Act& dst) {
+    add_ingest(&tp->pl, name, s, dst);
+    tp->ingest.push_back(tp->pl.ops.size() - 1);
+}
 
 // Add one block to a training plan: forward launches, statistics buffers, dgrad launches, wgrad.
 //   x / y: input and output views;   dy: gradient view of y;   dx: where the input gradient goes (base nullptr: none);
 //   dx_add: extra gradient added to dx (skip half of a concat gradient), base nullptr: none.
+//   fold_in: the caller tensor x is ingested from (first blocks). Without an input gradient, the forward conv may then read
+//   a second, K-folded copy of it (the inference plan's first-layer layout, 10-20x faster on the 7x7 / 6-channel layer)
+//   written by one more ingest launch; the backward (wgrad) reads the plain NHWC copy.
 static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const Layer& L, const Act& x, const Act& y, const Act& dy,
                            const Act& dx, const Act& dx_add, bool want_wgrad, bool in_hw1, size_t* ws_need, float* y_f32 = nullptr,
-                           const FoldIn* fold = nullptr) {
+                           const IngestSpec* fold_in = nullptr) {
     TrainState* ts = train_state(ctx);
     TBlock b;
     b.li = li; b.L = L; b.x = x; b.y = y; b.dy = dy; b.dx = dx; b.dx_add = dx_add; b.y_f32 = y_f32;
@@ -369,34 +369,23 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
     cudaStream_t st = nullptr;
     // ---- forward weights + launches ----
     if ((int)tp->wf.layers.size() <= li) { tp->wf.layers.resize(li + 1); tp->wd.layers.resize(li + 1); }
-    ctx->pack_rec = &tp->pack_jobs; ctx->fold_rec = &tp->fold_jobs; ctx->pack_fold_rec = &tp->pack_fold_jobs;
-    const bool use_fold_fwd = fold && fold->on && tp->allow_fold && !dx.base;
-    if (use_fold_fwd) ctx->use_fold = true;
-    int r = load_layer(ctx, &tp->wf.layers[li], L, b.W, b.bn ? nullptr : b.b, nullptr, nullptr, nullptr, nullptr, in_hw1, use_fold_fwd, st);
-    ctx->pack_fold_rec = nullptr;
-    if (r == W2L_OK && dx.base) {
+    const bool fold = fold_in && ctx->use_fold && ctx->use_patch && !dx.base;
+    CKR(load_layer(ctx, &tp->wf.layers[li], L, b.W, b.bn ? nullptr : b.b, nullptr, nullptr, nullptr, nullptr, in_hw1, fold,
+                   &tp->repack, st));
+    if (dx.base) {
         b.Ld = dgrad_layer(L, x.H, x.W, y.H, y.W, ctx->use_tma_epi);
-        r = load_dgrad_layer(ctx, &tp->wd.layers[li], L, b.Ld, b.W, st);
+        CKR(load_dgrad_layer(ctx, &tp->wd.layers[li], L, b.Ld, b.W, &tp->repack, st));
     }
-    ctx->pack_rec = nullptr; ctx->fold_rec = nullptr;
-    if (r != W2L_OK) { if (use_fold_fwd) ctx->use_fold = false; return r; }
     Act conv_out = y;
     if (b.bn) { CKR(tp_act(tp, &b.z, y.N, y.H, y.W, L.cout)); conv_out = b.z; }
     Act x_fwd = x;
-    if (use_fold_fwd && tp->wf.layers[li].ph[0].fold) {
-        int rr = plan_input_act(&tp->pl, &x_fwd, x.N, x.H, x.W, L.cin, tp->wf.layers[li], L);
-        if (rr != W2L_OK) { ctx->use_fold = false; return rr; }
-        add_ingest(&tp->pl, "ingest.fold", fold->src_id, x_fwd, fold->B, fold->C, fold->sB, fold->sC, fold->sT, fold->y_off, fold->Wsrc);
-        tp->pl.ops.back().ip.cgrp = fold->cgrp; tp->pl.ops.back().ip.sG = fold->sG;
-        tp->ingest.push_back(tp->pl.ops.size() - 1);
+    if (tp->wf.layers[li].ph[0].fold) {
+        CKR(plan_input_act(&tp->pl, &x_fwd, x.N, x.H, x.W, L.cin, tp->wf.layers[li], L));
+        add_train_ingest(tp, "ingest.fold", *fold_in, x_fwd);
         b.x_fold = x_fwd; b.fold_cp = tp->wf.layers[li].ph[0].Cp;
     }
     b.fwd0 = tp->pl.ops.size();
-    {
-        const int rr = emit_block(ctx, &tp->pl, tp->wf, li, L, x_fwd, conv_out, nullptr, false, 1, 1, b.bn ? ACT_NONE : -1);
-        if (use_fold_fwd) ctx->use_fold = false;
-        CKR(rr);
-    }
+    CKR(emit_block(ctx, &tp->pl, tp->wf, li, L, x_fwd, conv_out, nullptr, false, 1, 1, b.bn ? ACT_NONE : -1));
     b.fwd1 = tp->pl.ops.size();
     for (size_t i = b.fwd0; i < b.fwd1; ++i) tp->fwd_flops += tp->pl.ops[i].flops;
     // ---- statistics / reduction buffers ----
@@ -459,7 +448,7 @@ static void train_block_info(const w2l_ctx* ctx, const TrainPlan* tp, const TBlo
 //   its gradient view (base nullptr: allocate dense ones, returned through out / dout)
 static int add_train_chain(w2l_ctx* ctx, TrainPlan* tp, int net, const std::vector<Layer>& layers, const std::vector<int>& idx,
                            Act x0, Act dx0, Act dx0_add, const Act* last, const Act* dlast, bool want_wgrad, size_t* ws_need,
-                           Act* out, Act* dout, float* last_f32 = nullptr, const FoldIn* fold = nullptr) {
+                           Act* out, Act* dout, float* last_f32 = nullptr, const IngestSpec* fold_in = nullptr) {
     // values and gradients of every block output first (the gradient view of y[k] is the dx of block k+1)
     std::vector<Act> ys(idx.size()), dys(idx.size());
     int H = x0.H, W = x0.W;
@@ -483,17 +472,11 @@ static int add_train_chain(w2l_ctx* ctx, TrainPlan* tp, int net, const std::vect
         const Act& dx = k == 0 ? dx0 : dys[k - 1];
         const bool hw1 = L.kind == W2L_BLOCK_CONVT_BN_RELU && x.H == 1 && x.W == 1;
         CKR(add_train_block(ctx, tp, net, idx[k], L, x, ys[k], dys[k], dx, k == 0 ? dx0_add : none, want_wgrad, hw1, ws_need,
-                            k + 1 == idx.size() ? last_f32 : nullptr, k == 0 ? fold : nullptr));
+                            k + 1 == idx.size() ? last_f32 : nullptr, k == 0 ? fold_in : nullptr));
     }
     if (out) *out = ys.back();
     if (dout) *dout = dys.back();
     return W2L_OK;
-}
-
-static void add_train_ingest(TrainPlan* tp, const char* name, int src_id, const Act& dst, int B, int C, long long sB, long long sC,
-                             long long sT, int y_off, int Wsrc) {
-    add_ingest(&tp->pl, name, src_id, dst, B, C, sB, sC, sT, y_off, Wsrc);
-    tp->ingest.push_back(tp->pl.ops.size() - 1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -506,47 +489,35 @@ static int build_generator_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_ne
     Act faceIn, melIn, none;
     CKR(tp_act(tp, &faceIn, N, 96, 96, 16));
     CKR(tp_act(tp, &melIn, N, 80, 16, 16));
-    FoldIn fmel, fface;
-    fmel.on = fface.on = true;
-    if (T > 0) {
-        add_train_ingest(tp, "ingest.mel", 0, melIn, B, 1, (long long)T * 1280, 1280, 1280, 0, 16);
-        add_train_ingest(tp, "ingest.face", 1, faceIn, B, 6, (long long)6 * T * 9216, (long long)T * 9216, 9216, 0, 96);
-        fmel.src_id = 0; fmel.B = B; fmel.C = 1; fmel.sB = (long long)T * 1280; fmel.sC = 1280; fmel.sT = 1280; fmel.Wsrc = 16;
-        fface.src_id = 1; fface.B = B; fface.C = 6; fface.sB = (long long)6 * T * 9216; fface.sC = (long long)T * 9216; fface.sT = 9216; fface.Wsrc = 96;
-    } else {
-        add_train_ingest(tp, "ingest.mel", 0, melIn, N, 1, 1280, 1280, 0, 0, 16);
-        add_train_ingest(tp, "ingest.face", 1, faceIn, N, 6, 6 * 9216, 9216, 0, 0, 96);
-        fmel.src_id = 0; fmel.B = N; fmel.C = 1; fmel.sB = 1280; fmel.sC = 1280; fmel.Wsrc = 16;
-        fface.src_id = 1; fface.B = N; fface.C = 6; fface.sB = 6 * 9216; fface.sC = 9216; fface.Wsrc = 96;
-    }
-    const int hw[7] = {1, 3, 6, 12, 24, 48, 96};
-    const int dec_c[7] = {512, 512, 512, 384, 256, 128, 64};
-    const int skip_c[7] = {512, 512, 256, 128, 64, 32, 16};
+    IngestSpec mel, face;
+    generator_inputs(B, T, &mel, &face);
+    add_train_ingest(tp, "ingest.mel", mel, melIn);
+    add_train_ingest(tp, "ingest.face", face, faceIn);
     Act D[7], dD[7];   // [decoder output | encoder skip] and its gradient (wav2lip.py:108)
     for (int k = 0; k < 7; ++k) {
-        CKR(tp_act(tp, &D[k], N, hw[k], hw[k], dec_c[k] + skip_c[k]));
-        CKR(tp_act(tp, &dD[k], N, hw[k], hw[k], dec_c[k] + skip_c[k]));
+        CKR(tp_act(tp, &D[k], N, g.hw[k], g.hw[k], g.dec_c[k] + g.skip_c[k]));
+        CKR(tp_act(tp, &dD[k], N, g.hw[k], g.hw[k], g.dec_c[k] + g.skip_c[k]));
     }
     // audio encoder
     Act AE, dAE;
-    CKR(add_train_chain(ctx, tp, net, g.layers, g.audio_enc, melIn, none, none, nullptr, nullptr, true, ws_need, &AE, &dAE, nullptr, &fmel));
+    CKR(add_train_chain(ctx, tp, net, g.layers, g.audio_enc, melIn, none, none, nullptr, nullptr, true, ws_need, &AE, &dAE, nullptr, &mel));
     // face encoder: stage i ends in the skip half of D[6-i]; the gradient of a stage output is
     //   (input gradient of the next stage's first block) + (skip half of dD[6-i])  — the latter joins in that dgrad's epilogue
     Act x = faceIn, dx = none;
     Act G[7];          // total gradient of stage i's output
-    for (int i = 0; i < 6; ++i) CKR(tp_act(tp, &G[i], N, hw[6 - i], hw[6 - i], skip_c[6 - i]));
-    G[6] = dD[0].slice(dec_c[0], skip_c[0]);
+    for (int i = 0; i < 6; ++i) CKR(tp_act(tp, &G[i], N, g.hw[6 - i], g.hw[6 - i], g.skip_c[6 - i]));
+    G[6] = dD[0].slice(g.dec_c[0], g.skip_c[0]);
     for (int i = 0; i < 7; ++i) {
-        Act dst = D[6 - i].slice(dec_c[6 - i], skip_c[6 - i]);
-        Act add = i > 0 ? dD[6 - (i - 1)].slice(dec_c[6 - (i - 1)], skip_c[6 - (i - 1)]) : none;
+        Act dst = D[6 - i].slice(g.dec_c[6 - i], g.skip_c[6 - i]);
+        Act add = i > 0 ? dD[6 - (i - 1)].slice(g.dec_c[6 - (i - 1)], g.skip_c[6 - (i - 1)]) : none;
         CKR(add_train_chain(ctx, tp, net, g.layers, g.face_enc[i], x, dx, add, &dst, &G[i], true, ws_need, nullptr, nullptr, nullptr,
-                            i == 0 ? &fface : nullptr));
+                            i == 0 ? &face : nullptr));
         x = dst; dx = G[i];
     }
     // decoder
     x = AE; dx = dAE;
     for (int k = 0; k < 7; ++k) {
-        Act dst = D[k].slice(0, dec_c[k]), ddst = dD[k].slice(0, dec_c[k]);
+        Act dst = D[k].slice(0, g.dec_c[k]), ddst = dD[k].slice(0, g.dec_c[k]);
         CKR(add_train_chain(ctx, tp, net, g.layers, g.face_dec[k], x, dx, none, &dst, &ddst, true, ws_need, nullptr, nullptr));
         x = D[k]; dx = dD[k];
     }
@@ -567,14 +538,10 @@ static int build_syncnet_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_need
     Act faceIn, melIn, none;
     CKR(tp_act(tp, &faceIn, N, 48, 96, 16));
     CKR(tp_act(tp, &melIn, N, 80, 16, 16));
-    add_train_ingest(tp, "ingest.mel", 0, melIn, N, 1, 1280, 1280, 0, 0, 16);
-    if (tp->T > 0) {   // frames (B,3,T,96,96): lower half, frames stacked on channels (wav2lip_train.py:193-194)
-        const int T = tp->T;
-        add_train_ingest(tp, "ingest.frames", 1, faceIn, N, 3 * T, (long long)3 * T * 9216, (long long)T * 9216, 0, 48, 96);
-        tp->pl.ops.back().ip.cgrp = 3; tp->pl.ops.back().ip.sG = 9216;
-    } else {
-        add_train_ingest(tp, "ingest.face", 1, faceIn, N, 15, 15 * 4608, 4608, 0, 0, 96);
-    }
+    IngestSpec mel, face;
+    syncnet_inputs(N, tp->T, &mel, &face);
+    add_train_ingest(tp, "ingest.mel", mel, melIn);
+    add_train_ingest(tp, tp->T > 0 ? "ingest.frames" : "ingest.face", face, faceIn);
     void* p = nullptr;
     CKR(plan_alloc(&tp->pl, &p, (size_t)N * 512 * 4)); tp->fe_raw = (float*)p;
     CKR(plan_alloc(&tp->pl, &p, (size_t)N * 512 * 4)); tp->ae_raw = (float*)p;
@@ -592,7 +559,7 @@ static int build_disc_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_need, b
     const int N = tp->N, B = tp->B, T = tp->T, net = W2L_NET_DISC;
     Act in, none;
     CKR(tp_act(tp, &in, N, 48, 96, 16));
-    add_train_ingest(tp, "ingest.frames", 0, in, B, 3, (long long)3 * T * 9216, (long long)T * 9216, 9216, 48, 96);
+    add_train_ingest(tp, "ingest.frames", disc_input(B, T), in);
     if (input_grad) CKR(tp_act(tp, &tp->dframes_in, N, 48, 96, 16));
     std::vector<int> idx;
     for (size_t i = 0; i < d.layers.size(); ++i) idx.push_back((int)i);
@@ -617,17 +584,11 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
     std::unique_ptr<TrainPlan> tp(new TrainPlan());
     tp->net = net; tp->B = B; tp->T = T; tp->input_grad = input_grad;
     tp->N = (net == W2L_NET_SYNCNET) ? B : (T > 0 ? B * T : B);
-    // the specialised first-layer paths (K-folded input layouts) are inference-only: training keeps plain NHWC inputs,
-    // which is what the wgrad kernel reads
-    const bool s_fold = ctx->use_fold;
-    tp->allow_fold = s_fold && ctx->use_patch;
-    ctx->use_fold = false;
     size_t ws_need[2] = {0, 0};
     int r;
     if (net == W2L_NET_GENERATOR) r = build_generator_train_plan(ctx, tp.get(), ws_need);
     else if (net == W2L_NET_SYNCNET) r = build_syncnet_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
     else r = build_disc_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
-    ctx->use_fold = s_fold;
     for (int lane = 0; lane < 2 && r == W2L_OK; ++lane) {
         if (!ws_need[lane]) continue;
         void* p = nullptr;
@@ -645,20 +606,21 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
 // replay (training plans exist only on bf16 contexts, get_train_plan: every launch below is the bf16 instantiation)
 // ------------------------------------------------------------------------------------------------
 static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
-    if (!tp->pack_jobs.empty()) {
+    const std::vector<PackParams>& jobs = tp->repack.pack;
+    if (!jobs.empty()) {
         if (!tp->pack_dev) {   // job table + block map, built once per plan
             std::vector<int> blk_job, blk_first;
-            for (size_t j = 0; j < tp->pack_jobs.size(); ++j) {
-                const PackParams& pp = tp->pack_jobs[j];
+            for (size_t j = 0; j < jobs.size(); ++j) {
+                const PackParams& pp = jobs[j];
                 const long long total = (long long)pp.ntaps * pp.cout_pad * pp.cin_pad;
                 blk_first.push_back((int)blk_job.size());
                 for (long long b = 0; b < (total + 4095) / 4096; ++b) blk_job.push_back((int)j);
             }
             void* d = nullptr;
-            CKR(plan_alloc(&tp->pl, &d, tp->pack_jobs.size() * sizeof(PackParams))); tp->pack_dev = (PackParams*)d;
+            CKR(plan_alloc(&tp->pl, &d, jobs.size() * sizeof(PackParams))); tp->pack_dev = (PackParams*)d;
             CKR(plan_alloc(&tp->pl, &d, blk_job.size() * 4)); tp->pack_blk_job = (int*)d;
             CKR(plan_alloc(&tp->pl, &d, blk_first.size() * 4)); tp->pack_blk_first = (int*)d;
-            CK(cudaMemcpy(tp->pack_dev, tp->pack_jobs.data(), tp->pack_jobs.size() * sizeof(PackParams), cudaMemcpyHostToDevice));
+            CK(cudaMemcpy(tp->pack_dev, jobs.data(), jobs.size() * sizeof(PackParams), cudaMemcpyHostToDevice));
             CK(cudaMemcpy(tp->pack_blk_job, blk_job.data(), blk_job.size() * 4, cudaMemcpyHostToDevice));
             CK(cudaMemcpy(tp->pack_blk_first, blk_first.data(), blk_first.size() * 4, cudaMemcpyHostToDevice));
             tp->pack_blocks = (int)blk_job.size();
@@ -666,33 +628,17 @@ static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
         pack_multi_kernel<true><<<tp->pack_blocks, 256, 0, st>>>(tp->pack_dev, tp->pack_blk_job, tp->pack_blk_first);
         ctx->launches++;
     }
-    for (const PackFoldParams& fp : tp->pack_fold_jobs) {
+    for (const PackFoldParams& fp : tp->repack.pack_fold) {
         const size_t n = (size_t)fp.kh * fp.cout_pad * fp.kfold;
         const int blocks = (int)std::min<size_t>((n + 255) / 256, 4096);
         pack_fold_kernel<true><<<blocks, 256, 0, st>>>(fp);
         ctx->launches++;
     }
-    for (const FoldJob& f : tp->fold_jobs) {
+    for (const FoldJob& f : tp->repack.fold) {
         fold_bn_kernel<<<(f.n_pad + 127) / 128, 128, 0, st>>>(f.bias, nullptr, nullptr, nullptr, nullptr, 1e-5f, f.cout, f.reps, f.n_pad, f.scale, f.shift);
         ctx->launches++;
     }
     CK(cudaGetLastError());
-    return W2L_OK;
-}
-
-static int launch_ingest(w2l_ctx* ctx, const Op& op, const void* src, cudaStream_t st) {
-    IngestParams ip = op.ip;
-    ip.src = (const float*)src;
-    const long long total = (long long)ip.N * ip.H * ip.W;
-    const bool vec4 = ip.lo_off == 0 && ((ip.W | ip.Wsrc) & 3) == 0 && ((ip.sB | ip.sC | ip.sT | ip.sG) & 3) == 0 && (((uintptr_t)ip.src) & 15) == 0;
-    if (vec4) {
-        const int blocks = (int)std::min<long long>((total / 4 + 255) / 256, ctx->num_sms * 16);
-        ingest4_kernel<true><<<blocks, 256, 0, st>>>(ip);
-    } else {
-        const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-        ingest_kernel<true><<<blocks, 256, 0, st>>>(ip);
-    }
-    ctx->launches++;
     return W2L_OK;
 }
 

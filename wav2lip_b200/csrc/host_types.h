@@ -168,12 +168,12 @@ struct Plan {
 };
 
 struct FoldJob { const float* bias; int cout, reps, n_pad; float* scale; float* shift; };  // nonorm blocks: shift = conv bias
+// the launches that pack a training plan's 16-bit weight slabs from the fp32 master tensors, replayed after every
+// optimizer step (repack_weights)
+struct RepackLog { std::vector<PackParams> pack; std::vector<PackFoldParams> pack_fold; std::vector<FoldJob> fold; };
 struct TrainState;  // host_train.cuh
 
 struct w2l_ctx {
-    std::vector<PackParams>* pack_rec = nullptr;  // when set, pack_taps records its jobs (training re-packs every step)
-    std::vector<FoldJob>* fold_rec = nullptr;
-    std::vector<PackFoldParams>* pack_fold_rec = nullptr;
     TrainState* train = nullptr;
     int device = 0;
     bool bf16 = false;

@@ -17,8 +17,10 @@ static int need(const TensorMap& tm, const std::string& name, int64_t numel, con
     return W2L_OK;
 }
 
+// log != nullptr (training): the job is also recorded there, to be replayed after every optimizer step
 static int pack_taps(w2l_ctx* ctx, PackedW* pw, const float* src, int cout, int cin, int kh, int kw, bool transposed,
-                     const std::vector<std::pair<int, int>>& rs, int cout_pad_to, cudaStream_t st, uint16_t* dst_override = nullptr) {
+                     const std::vector<std::pair<int, int>>& rs, int cout_pad_to, RepackLog* log, cudaStream_t st,
+                     uint16_t* dst_override = nullptr) {
     PackParams pp;
     memset(&pp, 0, sizeof(pp));
     pp.src = src;
@@ -43,7 +45,7 @@ static int pack_taps(w2l_ctx* ctx, PackedW* pw, const float* src, int cout, int 
         pw->nslabs = pp.ntaps * planes;
     }
     const int blocks = (int)std::min<size_t>((n + 255) / 256, 4096);
-    if (ctx->pack_rec) ctx->pack_rec->push_back(pp);  // training: the same job is replayed after every optimizer step
+    if (log) log->pack.push_back(pp);
     for (int pl_ = 0; pl_ < planes; ++pl_) {  // hi slabs, then (split-operand mode) the lo slabs w - fp16(w)
         pp.lo = pl_;
         if (ctx->bf16) pack_w_kernel<true><<<blocks, 256, 0, st>>>(pp);
@@ -67,12 +69,14 @@ static void free_layer(LayerW& lw) {
 }
 
 // Pack one block's parameters. in_hw1: the block is applied to a 1x1 input (enables the GEMM form of convT).
+//   fold: the block may read a K-folded input (first layers fed by the ingest kernel);  log: see pack_taps
 static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, const float* bias, const float* gamma,
-                      const float* beta, const float* mean, const float* var, bool in_hw1, bool first_layer, cudaStream_t st) {
+                      const float* beta, const float* mean, const float* var, bool in_hw1, bool fold, RepackLog* log,
+                      cudaStream_t st) {
     free_layer(*lw);
     const int pad_to = 16;
     int reps = 1;
-    if (first_layer && ctx->use_fold && L.kind != W2L_BLOCK_CONVT_BN_RELU && L.cin <= 16 && L.kw >= 3 && (L.sw == 1 || L.sw == 2)) {
+    if (fold && L.kind != W2L_BLOCK_CONVT_BN_RELU && L.cin <= 16 && L.kw >= 3 && (L.sw == 1 || L.sw == 2)) {
         // tiny-Cin first layer: fold the kw horizontal taps into K (one K row per filter row r)
         PackedW pw;
         pw.fold = true;
@@ -91,7 +95,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         fp.src = W; fp.dst = pw.w; fp.kh = L.kh; fp.kw = L.kw; fp.cout = L.cout; fp.cin = L.cin;
         fp.cout_pad = pw.cout_pad; fp.kfold = pw.kfold; fp.Cp = pw.Cp;
         const int blocks = (int)std::min<size_t>((n + 255) / 256, 4096);
-        if (ctx->pack_fold_rec) ctx->pack_fold_rec->push_back(fp);
+        if (log) log->pack_fold.push_back(fp);
         if (ctx->bf16) pack_fold_kernel<true><<<blocks, 256, 0, st>>>(fp);
         else pack_fold_kernel<false><<<blocks, 256, 0, st>>>(fp);
         ctx->launches++;
@@ -102,7 +106,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         PackedW pw;
         for (int r = 0; r < L.kh; ++r)
             for (int s = 0; s < L.kw; ++s) { rs.push_back({r, s}); pw.dy.push_back((signed char)(r - L.ph)); pw.dx.push_back((signed char)(s - L.pw)); }
-        CKR(pack_taps(ctx, &pw, W, L.cout_real > 0 ? L.cout_real : L.cout, L.cin, L.kh, L.kw, false, rs, pad_to, st));
+        CKR(pack_taps(ctx, &pw, W, L.cout_real > 0 ? L.cout_real : L.cout, L.cin, L.kh, L.kw, false, rs, pad_to, log, st));
         lw->ph.push_back(pw);
     } else if (in_hw1 && !ctx->x2 && L.sh == 1 && L.sw == 1 && L.ph == 0 && L.pw == 0) {
         // out[n, y, x, co] = sum_ci in[n, ci] * W[ci, co, y, x]  -> GEMM with columns (y, x, co)
@@ -120,7 +124,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         for (int r = 0; r < L.kh; ++r)
             for (int s = 0; s < L.kw; ++s) {
                 std::vector<std::pair<int, int>> rs = {{r, s}};
-                CKR(pack_taps(ctx, nullptr, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, st,
+                CKR(pack_taps(ctx, nullptr, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st,
                               pw.w + (size_t)(r * L.kw + s) * L.cout * pw.cin_pad));
             }
         lw->ph.push_back(pw);
@@ -141,7 +145,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
                     }
                 }
                 if (rs.empty()) return fail(W2L_EINVAL, "%s: empty transposed-conv phase", L.name.c_str());
-                CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, st));
+                CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
                 lw->ph.push_back(pw);
             }
         if (!ctx->x2 && L.cout == kCtBN && L.kh == 3 && L.kw == 3 && L.sh == 2 && L.sw == 2 && L.ph == 1 && L.pw == 1 && L.out_pad == 1) {
@@ -154,7 +158,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
                                                    {0, 0}};                          // shift (1,1): phase 11
             PackedW pw;
             for (int t = 0; t < 9; ++t) { pw.dy.push_back(0); pw.dx.push_back(0); }
-            CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, st));
+            CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
             lw->ph.push_back(pw);
             lw->has_all_taps = true;
         }
@@ -165,7 +169,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
     CKR(dev_alloc(&sh, (size_t)n_pad * 4));
     lw->scale = (float*)sc; lw->shift = (float*)sh; lw->n_scale = n_pad;
     fold_bn_kernel<<<(n_pad + 127) / 128, 128, 0, st>>>(bias, gamma, beta, mean, var, 1e-5f, L.cout_real > 0 ? L.cout_real : L.cout, reps, n_pad, lw->scale, lw->shift);
-    if (ctx->fold_rec && bias) ctx->fold_rec->push_back(FoldJob{bias, L.cout, reps, n_pad, lw->scale, lw->shift});
+    if (log && bias) log->fold.push_back(FoldJob{bias, L.cout, reps, n_pad, lw->scale, lw->shift});
     ctx->launches++;
     CK(cudaGetLastError());
     lw->loaded = true;

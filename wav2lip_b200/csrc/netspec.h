@@ -60,6 +60,11 @@ struct GeneratorSpec {
     std::vector<int> audio_enc;              // 13 blocks
     std::vector<std::vector<int>> face_dec;  // 7 stages
     int output_block0;
+    // skip concatenation (wav2lip.py:108): decoder stage k's output (dec_c[k] channels) is concatenated with the encoder
+    // feature of the same resolution hw[k] (skip_c[k] channels); stage k + 1 reads both
+    int hw[7] = {1, 3, 6, 12, 24, 48, 96};
+    int dec_c[7] = {512, 512, 512, 384, 256, 128, 64};
+    int skip_c[7] = {512, 512, 256, 128, 64, 32, 16};
 };
 
 inline GeneratorSpec build_generator_spec() {
@@ -92,8 +97,7 @@ inline GeneratorSpec build_generator_spec() {
         for (size_t k = b; k < L.size(); ++k) g.audio_enc.push_back((int)k);
     }
     // decoder: input width of stage k = (own output of stage k-1) + (encoder skip of the same resolution)
-    const int dec_c[7] = {512, 512, 512, 384, 256, 128, 64};
-    const int skip_c[7] = {512, 512, 256, 128, 64, 32, 16};
+    const int *dec_c = g.dec_c, *skip_c = g.skip_c;
     const int dec_res[7] = {0, 1, 2, 2, 2, 2, 2};
     {
         const size_t b = L.size();

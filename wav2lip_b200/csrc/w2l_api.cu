@@ -207,7 +207,7 @@ int w2l_load_weights(w2l_ctx* ctx, int net, int n_tensors, const char* const* na
         // the generator's 16->32 stride-2 block reads a dense zero-bordered copy of the first block's output (written by
         // the patch kernel's second TMA store) through the same overlapping-window trick
         if (net == W2L_NET_GENERATOR && L.name == "face_encoder_blocks.1.0" && ctx->use_patch && ctx->use_fold && ctx->use_fold_s2) first = true;
-        CKR(load_layer(ctx, &nw.layers[i], L, W, b, gm, be, m, v, hw1, first, st));
+        CKR(load_layer(ctx, &nw.layers[i], L, W, b, gm, be, m, v, hw1, first && ctx->use_fold, nullptr, st));
     }
     if (nw.head_w) { cudaFree(nw.head_w); nw.head_w = nullptr; }
     if (nw.head_b) { cudaFree(nw.head_b); nw.head_b = nullptr; }
@@ -664,29 +664,42 @@ int w2l_disc_forward(w2l_ctx* ctx, const float* frames, float* prob, int B, int 
     return run_plan(ctx, pl, frames, nullptr, prob, nullptr, (cudaStream_t)stream);
 }
 
+// The block of a single-block entry, from the caller's description: every field is checked here, before anything is
+// allocated or launched.  Ho / Wo: the output size on an N x H x W input.
+static int block_from_info(const w2l_layer_info* spec, const char* name, int N, int H, int W, Layer* L, int* Ho, int* Wo) {
+    if (N <= 0 || H <= 0 || W <= 0) return fail(W2L_EINVAL, "bad shape N=%d H=%d W=%d", N, H, W);
+    const w2l_layer_info& s = *spec;
+    if (s.kind < W2L_BLOCK_CONV_BN_RELU || s.kind > W2L_BLOCK_CONV_RELU) return fail(W2L_EINVAL, "unknown block kind %d", s.kind);
+    if (s.cin < 1) return fail(W2L_EINVAL, "cin %d < 1", s.cin);
+    if (s.cout <= 0 || s.cout % 16 != 0) return fail(W2L_EINVAL, "cout %d: must be a positive multiple of 16", s.cout);
+    if (s.kh < 1 || s.kw < 1 || (long long)s.kh * s.kw > kMaxTaps)
+        return fail(W2L_EINVAL, "kernel %dx%d: needs 1 to %d taps", s.kh, s.kw, kMaxTaps);
+    if (s.sh < 1 || s.sw < 1) return fail(W2L_EINVAL, "stride %dx%d < 1", s.sh, s.sw);
+    if (s.ph < 0 || s.pw < 0 || s.out_pad < 0) return fail(W2L_EINVAL, "negative padding");
+    L->name = name;
+    L->kind = s.kind; L->cin = s.cin; L->cout = s.cout; L->kh = s.kh; L->kw = s.kw;
+    L->sh = s.sh; L->sw = s.sw; L->ph = s.ph; L->pw = s.pw; L->out_pad = s.out_pad; L->residual = s.residual != 0;
+    conv_out_dims(*L, H, W, Ho, Wo);
+    if (*Ho <= 0 || *Wo <= 0) return fail(W2L_EINVAL, "empty output");
+    if (L->residual && (L->cin != L->cout || *Ho != H || *Wo != W)) return fail(W2L_EINVAL, "residual needs same shape");
+    return W2L_OK;
+}
+
 int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float* x, int N, int H, int W,
                            const float* weight, const float* bias, const float* bn_w, const float* bn_b,
                            const float* bn_m, const float* bn_v, float* y, void* stream) {
     if (!ctx || !spec || !x || !weight || !y) return fail(W2L_EINVAL, "null argument");
-    if (N <= 0 || H <= 0 || W <= 0) return fail(W2L_EINVAL, "bad shape");
+    Layer L;
+    int Ho, Wo;
+    const std::string name(spec->name, strnlen(spec->name, sizeof(spec->name)));
+    CKR(block_from_info(spec, name.empty() ? "block" : name.c_str(), N, H, W, &L, &Ho, &Wo));
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    Layer L;
-    L.name = spec->name[0] ? spec->name : "block";
-    L.kind = spec->kind; L.cin = spec->cin; L.cout = spec->cout; L.kh = spec->kh; L.kw = spec->kw;
-    L.sh = spec->sh; L.sw = spec->sw; L.ph = spec->ph; L.pw = spec->pw; L.out_pad = spec->out_pad; L.residual = spec->residual != 0;
-    if (L.cout % 16 != 0) return fail(W2L_EINVAL, "cout must be a multiple of 16");
-    if (L.kh * L.kw > kMaxTaps) return fail(W2L_EINVAL, "kernel too large");
-    int Ho, Wo;
-    conv_out_dims(L, H, W, &Ho, &Wo);
-    if (Ho <= 0 || Wo <= 0) return fail(W2L_EINVAL, "empty output");
-    if (L.residual && (L.cin != L.cout || Ho != H || Wo != W)) return fail(W2L_EINVAL, "residual needs same shape");
-    const bool saved_fold = ctx->use_fold;
-    if (L.residual) ctx->use_fold = false;  // the residual is read from the block input: keep it in the plain NHWC layout
-    // a private one-block "network"
+    // a private one-block "network"; a residual is read from the block input, which then stays in the plain NHWC layout
     NetW scratch;
     scratch.layers.resize(1);
-    int r = load_layer(ctx, &scratch.layers[0], L, weight, bias, bn_w, bn_b, bn_m, bn_v, H == 1 && W == 1, true, st);
+    int r = load_layer(ctx, &scratch.layers[0], L, weight, bias, bn_w, bn_b, bn_m, bn_v, H == 1 && W == 1,
+                       ctx->use_fold && !L.residual, nullptr, st);
     Plan pl;
     pl.net = W2L_NET_DISC; pl.N = N; pl.B = N; pl.T = 0;
     pl.x2 = ctx->x2;
@@ -695,7 +708,7 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float
     if (r == W2L_OK) r = plan_act(&pl, &out, N, Ho, Wo, L.cout);
     ctx->last_block_kernels.clear();
     if (r == W2L_OK) {
-        add_ingest(&pl, "ingest.x", 0, in, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W);
+        add_ingest(&pl, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, in);
         r = emit_block(ctx, &pl, scratch, 0, L, in, out, L.residual ? &in : nullptr);
         if (r == W2L_OK) {
             for (const Op& op : pl.ops)
@@ -716,7 +729,6 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float
     }
     free_plan(&pl);
     free_layer(scratch.layers[0]);
-    ctx->use_fold = saved_fold;
     return r;
 }
 
@@ -1214,8 +1226,6 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
     CK(cudaEventCreate(&e0));
     CK(cudaEventCreate(&e1));
     int k = 0;
-    const bool pdl = ctx->use_pdl;
-    ctx->use_pdl = false;
     auto timed = [&](const std::string& name, double flops, const std::function<int()>& fn) -> int {
         if (k >= cap) return W2L_OK;
         CKR(fn());
@@ -1236,7 +1246,7 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
         double f = 0;
         for (size_t i = b.fwd0; i < b.fwd1; ++i) f += tp->pl.ops[i].flops;
         // forward conv only, then the statistics + normalise passes (running averages untouched)
-        r = timed(b.L.name + " fwd", f, [&]() -> int { for (size_t i = b.fwd0; i < b.fwd1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st)); return W2L_OK; });
+        r = timed(b.L.name + " fwd", f, [&]() -> int { for (size_t i = b.fwd0; i < b.fwd1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; });
         if (r != W2L_OK) break;
         if (b.bn) {
             TBlock c = b; c.fwd0 = c.fwd1 = 0;
@@ -1251,15 +1261,14 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
         if (b.dg1 > b.dg0) {
             double fd = 0;
             for (size_t i = b.dg0; i < b.dg1; ++i) fd += tp->pl.ops[i].flops;
-            r = timed(b.L.name + " dgrad", fd, [&]() -> int { for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st)); return W2L_OK; });
+            r = timed(b.L.name + " dgrad", fd, [&]() -> int { for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; });
             if (r != W2L_OK) break;
         }
         if (b.wg.on) {
-            r = timed(b.L.name + " wgrad", b.wg.flops, [&]() -> int { return launch_wgrad(ctx, tp, b, false, st); });
+            r = timed(b.L.name + " wgrad", b.wg.flops, [&]() -> int { return launch_wgrad(ctx, tp, b, false, st, false); });
             if (r != W2L_OK) break;
         }
     }
-    ctx->use_pdl = pdl;
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     return r == W2L_OK ? k : r;
@@ -1272,16 +1281,11 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
                          float* dw, float* db, float* dgamma, float* dbeta, void* stream) {
     if (!ctx || !spec || !x || !weight || !y) return fail(W2L_EINVAL, "null argument");
     if (!ctx->bf16) return fail(W2L_ESTATE, "training runs with bf16 operands: create the context with W2L_PREC_BF16");
+    Layer L;
+    int Ho, Wo;
+    CKR(block_from_info(spec, "block", N, H, W, &L, &Ho, &Wo));   // the name its tensors are bound under below
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    Layer L;
-    L.name = "block";
-    L.kind = spec->kind; L.cin = spec->cin; L.cout = spec->cout; L.kh = spec->kh; L.kw = spec->kw;
-    L.sh = spec->sh; L.sw = spec->sw; L.ph = spec->ph; L.pw = spec->pw; L.out_pad = spec->out_pad; L.residual = spec->residual != 0;
-    if (L.cout % 16 != 0) return fail(W2L_EINVAL, "cout must be a multiple of 16");
-    int Ho, Wo;
-    conv_out_dims(L, H, W, &Ho, &Wo);
-    if (Ho <= 0 || Wo <= 0) return fail(W2L_EINVAL, "empty output");
     TrainState* ts = train_state(ctx);
     CKR(ensure_train_scratch(ctx, 1, 1));
     const int slot = W2L_NET_DISC;
@@ -1299,8 +1303,6 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     }
     TrainPlan tp;
     tp.net = slot; tp.N = N; tp.B = N; tp.T = 0;
-    const bool s_fold = ctx->use_fold;
-    ctx->use_fold = false;
     Act xin, dxin, yv, dyv, none;
     size_t ws_need[2] = {0, 0};
     int r = tp_act(&tp, &xin, N, H, W, round_up(L.cin, 16));
@@ -1308,12 +1310,11 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     if (r == W2L_OK) r = tp_act(&tp, &yv, N, Ho, Wo, L.cout);
     if (r == W2L_OK) r = tp_act(&tp, &dyv, N, Ho, Wo, L.cout);
     if (r == W2L_OK) {
-        add_train_ingest(&tp, "ingest.x", 0, xin, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W);
-        add_train_ingest(&tp, "ingest.dy", 1, dyv, N, L.cout, (long long)L.cout * Ho * Wo, (long long)Ho * Wo, 0, 0, Wo);
+        add_train_ingest(&tp, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, xin);
+        add_train_ingest(&tp, "ingest.dy", IngestSpec{1, N, L.cout, (long long)L.cout * Ho * Wo, (long long)Ho * Wo, 0, 0, Wo}, dyv);
         r = add_train_block(ctx, &tp, slot, 0, L, xin, yv, dyv, dx ? dxin : none, none, dw != nullptr,
                             L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, ws_need);
     }
-    ctx->use_fold = s_fold;
     if (r == W2L_OK && ws_need[0]) { void* p = nullptr; r = plan_alloc(&tp.pl, &p, ws_need[0]); tp.wg_ws[0] = (float*)p; }
     if (r == W2L_OK) {
         cudaError_t e = cudaDeviceSynchronize();
