@@ -220,7 +220,10 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec,
                            float* y_dev, void* stream);
 
 /* Debug/test aid: copy the output of block `layer` (index into the net's table) of the LAST
- * forward of `net` to y (N,cout,H,W) fp32.  *h,*w,*c receive the dims (any may be NULL). */
+ * forward of `net` to y (N,cout,H,W) fp32.  *h,*w,*c receive the dims (any may be NULL).
+ * W2L_NET_S3FD also exports its glue ops after the 31 conv layers: 31..35 = the five max-pools (pool1..pool5),
+ * 36..38 = the three L2Norm outputs (conv3_3_norm, conv4_3_norm, conv5_3_norm).  The mbox heads (19..30) export all
+ * 16 stored channels; channels cout_real..15 are padding. */
 int w2l_debug_layer_output(w2l_ctx* ctx, int net, int layer, float* y_dev, int* n, int* c, int* h, int* w,
                            void* stream);
 

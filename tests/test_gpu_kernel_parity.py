@@ -14,13 +14,16 @@ Bars, derived rather than fitted, with mag = |scale|*conv(|x^|,|w^|) + |shift| +
               and, with >= 1e4 outputs, |mean(sign(ref) * (y - ref) / ulp16(ref))| <= 0.05 over the elements with
               |ref| > 2^-16 * mag (a truncating conversion gives about -0.5; elements within the accumulation error
               of zero are left out because a ReLU can move them by a whole value, not by a rounding step)
-  F32X        |y - ref| <= 2^-15 * mag     (split operands carry ~22 bits: about 2^-16 is expected, a dropped
-              x_lo*w_hi / x_hi*w_lo pass or residual lo plane costs about 2^-12)
+  F32X        |y - ref| <= 2^-15 * mag + lo_step(max(|y|,|ref|))     (split operands carry ~22 bits: about 2^-16 is
+              expected, a dropped x_lo*w_hi / x_hi*w_lo pass or residual lo plane costs about 2^-12; lo_step is the
+              rounding of the fp16 lo plane, ~2^-22 |y|, down to 2^-25 absolute where lo is subnormal)
 Every case also runs twice (bit-identical: inference has no atomics), leaves the fp16 range flag clear, and asserts
-the kernel family / BN / BK / MT / staged epilogue / fold that w2l_debug_plan_kernels reports for it.
+the kernel family / BN / BK / MT / staged epilogue / fold that w2l_debug_plan_kernels reports for it.  The S3FD cases use
+its conv + ReLU and plain (no activation) kinds, which have no BatchNorm: scale 1, shift = conv bias.
 
 Measured on one H100 SXM (80 GB, 700 W).  Values near 1 in F16 / BF16 are single last-bit flips where the
-accumulation term is small; the largest |bias| over all cases was 0.008 ulp; F32X reaches at most 0.06 of its bar.
+accumulation term is small; the largest |bias| over all cases was 0.008 ulp; F32X reaches at most 0.06 of its bar except
+on fc6 (0.48: its border outputs are the bias alone, bounded by the lo-plane term).
 max err/bar in F16 and BF16 (default and generic-only dispatch), and in F32X err/bar and err/mag:
   case                                                  f16  bf16  f32x    err/mag
   gen 7x7 6->16 96x96                                  0.91  0.98  0.033  1.0e-06
@@ -76,6 +79,27 @@ max err/bar in F16 and BF16 (default and generic-only dispatch), and in F32X err
   disc 512 3x3 6x6                                     0.73  0.95  0.053  1.6e-06
   disc 512 3x3 pad0 -> 1x1                             0.64  0.10  0.048  1.5e-06
   disc 512 1x1                                         0.39  0.07  0.017  5.1e-07
+  s3fd conv1_1 3->64 96x128                            0.97  0.95  0.031  9.5e-07
+  s3fd conv1_2 64 96x128                               0.91  0.98  0.024  7.4e-07
+  s3fd conv2_1 64->128 48x64                           0.90  0.98  0.024  7.2e-07
+  s3fd conv2_2 128 48x64                               0.88  0.98  0.035  1.1e-06
+  s3fd conv3_1 128->256 24x32                          0.88  0.98  0.030  9.1e-07
+  s3fd conv3_2 256 37x52                               0.83  0.97  0.045  1.4e-06
+  s3fd conv4_1 256->512 12x16                          0.79  0.95  0.040  1.2e-06
+  s3fd conv4_2 512 9x13                                0.83  0.88  0.054  1.6e-06
+  s3fd conv5_2 512 3x4                                 0.66  0.91  0.039  1.2e-06
+  s3fd fc6 512->1024 k3 p3 3x4                         0.81  0.97  0.478  5.1e-05
+  s3fd fc6 512->1024 k3 p3 1x1 -> 5x5                  0.89  0.89  0.478  5.1e-05
+  s3fd fc7 1024 1x1 7x8                                0.88  0.97  0.037  1.1e-06
+  s3fd conv6_1 1024->256 1x1 7x8                       0.79  0.97  0.036  1.1e-06
+  s3fd conv6_2 256->512 s2 7x8                         0.78  0.93  0.032  9.7e-07
+  s3fd conv6_2 256->512 s2 5x5 -> 3x3                  0.85  0.94  0.035  1.1e-06
+  s3fd conv7_1 512->128 1x1 4x4                        0.84  0.00  0.025  7.6e-07
+  s3fd conv7_2 128->256 s2 4x4                         0.72  0.00  0.020  6.0e-07
+  s3fd conv7_2 128->256 s2 3x3 -> 2x2                  0.79  0.01  0.017  5.2e-07
+  s3fd head plain 256->16 24x32                        0.71  0.95  0.040  1.2e-06
+  s3fd head plain 512->16 12x16                        0.72  0.93  0.041  1.2e-06
+  s3fd head plain 1024->16 7x8                         0.65  0.26  0.044  1.3e-06
   igemm BN16 BK16 48->48                               0.91  0.98
   igemm BN16 BK32 32->80                               0.89  0.97
   igemm BN16 BK64 64->48                               0.88  0.96
@@ -191,6 +215,13 @@ def ulp16(a, prec):
     return torch.where(a == 0, torch.full_like(a, MIN_SUB[prec]), torch.clamp(u, min=MIN_SUB[prec]))
 
 
+def lo_step(a):
+    """F32X stores y as hi + lo in two fp16 planes, lo = fp16(y - hi): the lo rounding is at most half an fp16 step of a
+    value at most half an fp16 step of y.  About 2^-22 |y|; it matters only where fp16 makes lo subnormal (|y| < ~2^-3),
+    and there only when mag is tiny too (an output that is a bias alone, like fc6's padding-only border)."""
+    return 0.5 * ulp16(0.5 * ulp16(a, F16), F16)
+
+
 def _row_geom(row):
     kind, cin, cout, k, s, p, op, res = row
     return kind, cin, cout, O._pair(k), O._pair(s), O._pair(p), op, res
@@ -199,7 +230,7 @@ def _row_geom(row):
 def fold_bn(sd, prefix, kind):
     """(scale, shift) float64 from the fp32 parameters, as fold_bn_kernel folds them."""
     b = sd[f"{prefix}.conv_block.0.bias"].double()
-    if kind == "n":
+    if kind in ("n", "r", "p"):   # no BatchNorm: scale 1, shift = conv bias
         return torch.ones_like(b), b
     g = sd[f"{prefix}.conv_block.1.weight"].double()
     be = sd[f"{prefix}.conv_block.1.bias"].double()
@@ -228,7 +259,10 @@ def reference(x, sd, prefix, row, prec, round_out=True):
     if res:
         v = v + xr
         mag = mag + xr.abs()
-    v = F.leaky_relu(v, 0.01) if kind == "n" else F.relu(v)
+    if kind == "n":
+        v = F.leaky_relu(v, 0.01)
+    elif kind != "p":
+        v = F.relu(v)
     if prec != F32X and round_out:
         v = round16(v, prec)
     return v, mag
@@ -241,7 +275,7 @@ def compare(y, ref, mag, prec, what=""):
     assert torch.isfinite(y).all(), f"{what}: non-finite output"
     err = (y - ref).abs()
     if prec == F32X:
-        bar = ACC_X2 * mag
+        bar = ACC_X2 * mag + lo_step(torch.maximum(y.abs(), ref.abs()))
     else:
         bar = ulp16(torch.maximum(y.abs(), ref.abs()), prec) + ACC * mag
     ratio = (err / bar).max().item()
@@ -262,7 +296,7 @@ def compare(y, ref, mag, prec, what=""):
 # ------------------------------------------------------------------------------------------------------------------
 # one block through w2l_conv_block_forward on a private context
 # ------------------------------------------------------------------------------------------------------------------
-KIND = {"c": 0, "t": 1, "n": 2}
+KIND = {"c": 0, "t": 1, "n": 2, "p": 3, "r": 4}   # W2L_BLOCK_*
 
 
 def block_forward(ctx, row, x, sd, prefix="b"):
@@ -294,7 +328,8 @@ def block_forward(ctx, row, x, sd, prefix="b"):
 
 def _tensors(row, seed, N, H, W):
     g = torch.Generator().manual_seed(seed)
-    sd = O._block_tensors("b", row, g, 1.0)
+    # _block_tensors adds BatchNorm tensors for every kind but "n"; the plain and ReLU kinds have none
+    sd = O._block_tensors("b", ("n",) + tuple(row[1:]) if row[0] in ("r", "p") else row, g, 1.0)
     x = torch.rand((N, row[1], H, W), generator=g) * 2 - 0.5
     return sd, x
 
@@ -313,6 +348,14 @@ def _t(cin, cout, k, s, p, op=0):
 
 def _n(cin, cout, k, s, p):
     return ("n", cin, cout, k, s, p, 0, False)
+
+
+def _r(cin, cout, k, s, p):
+    return ("r", cin, cout, k, s, p, 0, False)
+
+
+def _p(cin, cout, k, s, p):
+    return ("p", cin, cout, k, s, p, 0, False)
 
 
 # every distinct block geometry of the generator, SyncNet and the disc (input N, H, W), default-dispatch kernel in F16
@@ -370,6 +413,33 @@ GEOMS = [
     ("disc 512 3x3 6x6", _n(512, 512, 3, 1, 1), 2, 6, 6, "I32.64e"),
     ("disc 512 3x3 pad0 -> 1x1", _n(512, 512, 3, 1, 0), 2, 3, 3, "I32.64e"),
     ("disc 512 1x1", _n(512, 512, 1, 1, 0), 2, 1, 1, "I32.64e"),
+]
+
+# every distinct S3FD layer geometry (conv + ReLU backbone, plain 16-channel heads) at sizes its plans produce: the
+# backbone of a 96x128 frame, the odd maps of 150x210, fc6 (k3 pad 3) on the 1x1 pool5 of a 32x32 frame, the stride-2
+# convs down to 3x3 and 2x2 inputs
+S3FD_GEOMS = [
+    ("s3fd conv1_1 3->64 96x128", _r(3, 64, 3, 1, 1), 2, 96, 128, "P64.32f"),
+    ("s3fd conv1_2 64 96x128", _r(64, 64, 3, 1, 1), 2, 96, 128, "P64.64"),
+    ("s3fd conv2_1 64->128 48x64", _r(64, 128, 3, 1, 1), 2, 48, 64, "I32.64e"),
+    ("s3fd conv2_2 128 48x64", _r(128, 128, 3, 1, 1), 2, 48, 64, "I32.64e"),
+    ("s3fd conv3_1 128->256 24x32", _r(128, 256, 3, 1, 1), 2, 24, 32, "I32.64e"),
+    ("s3fd conv3_2 256 37x52", _r(256, 256, 3, 1, 1), 1, 37, 52, "I32.64e"),
+    ("s3fd conv4_1 256->512 12x16", _r(256, 512, 3, 1, 1), 2, 12, 16, "I32.64e"),
+    ("s3fd conv4_2 512 9x13", _r(512, 512, 3, 1, 1), 1, 9, 13, "I32.64e"),
+    ("s3fd conv5_2 512 3x4", _r(512, 512, 3, 1, 1), 2, 3, 4, "I32.64e"),
+    ("s3fd fc6 512->1024 k3 p3 3x4", _r(512, 1024, 3, 1, 3), 2, 3, 4, "I32.64e"),
+    ("s3fd fc6 512->1024 k3 p3 1x1 -> 5x5", _r(512, 1024, 3, 1, 3), 3, 1, 1, "I32.64e"),
+    ("s3fd fc7 1024 1x1 7x8", _r(1024, 1024, 1, 1, 0), 2, 7, 8, "I32.64e"),
+    ("s3fd conv6_1 1024->256 1x1 7x8", _r(1024, 256, 1, 1, 0), 2, 7, 8, "I32.64e"),
+    ("s3fd conv6_2 256->512 s2 7x8", _r(256, 512, 3, 2, 1), 2, 7, 8, "I32.64e"),
+    ("s3fd conv6_2 256->512 s2 5x5 -> 3x3", _r(256, 512, 3, 2, 1), 3, 5, 5, "I32.64e"),
+    ("s3fd conv7_1 512->128 1x1 4x4", _r(512, 128, 1, 1, 0), 2, 4, 4, "I32.64e"),
+    ("s3fd conv7_2 128->256 s2 4x4", _r(128, 256, 3, 2, 1), 2, 4, 4, "I32.64e"),
+    ("s3fd conv7_2 128->256 s2 3x3 -> 2x2", _r(128, 256, 3, 2, 1), 3, 3, 3, "I32.64e"),
+    ("s3fd head plain 256->16 24x32", _p(256, 16, 3, 1, 1), 2, 24, 32, "I16.64e"),
+    ("s3fd head plain 512->16 12x16", _p(512, 16, 3, 1, 1), 2, 12, 16, "I16.64e"),
+    ("s3fd head plain 1024->16 7x8", _p(1024, 16, 3, 1, 1), 2, 7, 8, "I16.64e"),
 ]
 
 # cases aimed at the dispatch boundaries (default dispatch, F16 and BF16)
@@ -488,6 +558,13 @@ def test_block_geometry_matches_float64(case, mode):
     run_case(case, prec, off)
 
 
+@pytest.mark.parametrize("mode", GEOM_MODES, ids=GEOM_MODE_IDS)
+@pytest.mark.parametrize("case", S3FD_GEOMS, ids=[c[0] for c in S3FD_GEOMS])
+def test_s3fd_geometry_matches_float64(case, mode):
+    prec, off = mode
+    run_case(case, prec, off)
+
+
 @pytest.mark.parametrize("prec", [F16, BF16], ids=["f16", "bf16"])
 @pytest.mark.parametrize("case", DISPATCH, ids=[c[0] for c in DISPATCH])
 def test_dispatch_boundary_matches_float64(case, prec):
@@ -560,7 +637,7 @@ def test_every_reachable_instantiation_is_covered():
     assert len(table) == 2 * (12 + 2 + 9 + 1)
     seen = set()
     for prec in (F16, BF16):
-        for case in GEOMS + DISPATCH:
+        for case in GEOMS + S3FD_GEOMS + DISPATCH:
             for k in run_case(case, prec)["kernels"]:
                 seen.add((k["family"], k["bn"], k["bk"], k["mt"], k["bf16"]))
     missing = [(k["family"], k["bn"], k["bk"], k["mt"], k["bf16"]) for k in table

@@ -340,48 +340,88 @@ __global__ void disc_head_kernel(const uint16_t* x, const float* w, const float*
 }
 
 // ---- S3FD (face_detection/detection/sfd/net_s3fd.py) glue kernels ---------------------------------------------------------
-// F.max_pool2d(h, 2, 2) (net_s3fd.py:74,78,84,90,96): NHWC 16-bit, floor semantics, 8 channels per thread
+// Both read and write NHWC 16-bit activations with pixel pitch Cs.  lo_off > 0 (split-operand mode, Cs = 2C): every value
+// is hi + lo, the lo plane lo_off channels after the hi plane; both planes are read and both are written.
+
+__device__ __forceinline__ uint16_t half_of(const uint4& q, int j) {
+    const uint32_t w = (&q.x)[j >> 1];
+    return (uint16_t)((j & 1) ? (w >> 16) : (w & 0xFFFFu));
+}
+__device__ __forceinline__ uint4 pack8(const uint16_t* o) {
+    return make_uint4(o[0] | ((uint32_t)o[1] << 16), o[2] | ((uint32_t)o[3] << 16), o[4] | ((uint32_t)o[5] << 16),
+                      o[6] | ((uint32_t)o[7] << 16));
+}
+
+// F.max_pool2d(h, 2, 2) (net_s3fd.py:74,78,84,90,96): floor semantics, 8 channels per thread.  Split operands: the
+// window's largest hi + lo wins and both of its planes are copied, so the pool is exact in every mode.
 template <bool kBF16>
-__global__ void maxpool2_kernel(const uint16_t* in, uint16_t* out, int N, int H, int W, int C) {
+__global__ void maxpool2_kernel(const uint16_t* in, uint16_t* out, int N, int H, int W, int C, int Cs, int lo_off) {
     const int Ho = H >> 1, Wo = W >> 1, cg = C >> 3;
     const long long total = (long long)N * Ho * Wo * cg;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int g = (int)(i % cg);
         const int x = (int)((i / cg) % Wo), y = (int)((i / ((long long)cg * Wo)) % Ho), n = (int)(i / ((long long)cg * Wo * Ho));
-        const uint16_t* p = in + ((((long long)n * H + 2 * y) * W + 2 * x) * C) + g * 8;
-        const uint4 q[4] = {__ldg(reinterpret_cast<const uint4*>(p)), __ldg(reinterpret_cast<const uint4*>(p + C)),
-                            __ldg(reinterpret_cast<const uint4*>(p + (long long)W * C)), __ldg(reinterpret_cast<const uint4*>(p + (long long)W * C + C))};
+        const long long row = (long long)W * Cs;
+        const uint16_t* p = in + ((((long long)n * H + 2 * y) * W + 2 * x) * Cs) + g * 8;
+        const uint16_t* po[4] = {p, p + Cs, p + row, p + row + Cs};
+        uint4 q[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) q[k] = __ldg(reinterpret_cast<const uint4*>(po[k]));
+        uint16_t* d = out + ((((long long)n * Ho + y) * Wo + x) * Cs) + g * 8;
         uint16_t o[8];
+        if (lo_off > 0) {
+            uint4 l[4];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float m = -3.4e38f;
+            for (int k = 0; k < 4; ++k) l[k] = __ldg(reinterpret_cast<const uint4*>(po[k] + lo_off));
+            uint16_t ol[8];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const uint32_t w = (&q[k].x)[j >> 1];
-                m = fmaxf(m, from16<kBF16>((uint16_t)((j & 1) ? (w >> 16) : (w & 0xFFFFu))));
+            for (int j = 0; j < 8; ++j) {
+                int best = 0;
+                float m = from16<kBF16>(half_of(q[0], j)) + from16<kBF16>(half_of(l[0], j));
+#pragma unroll
+                for (int k = 1; k < 4; ++k) {
+                    const float v = from16<kBF16>(half_of(q[k], j)) + from16<kBF16>(half_of(l[k], j));
+                    if (v > m) { m = v; best = k; }
+                }
+                o[j] = half_of(q[best], j);
+                ol[j] = half_of(l[best], j);
             }
-            o[j] = to16<kBF16>(m);
+            *reinterpret_cast<uint4*>(d + lo_off) = pack8(ol);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float m = -3.4e38f;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) m = fmaxf(m, from16<kBF16>(half_of(q[k], j)));
+                o[j] = to16<kBF16>(m);
+            }
         }
-        uint4 r;
-        r.x = o[0] | ((uint32_t)o[1] << 16); r.y = o[2] | ((uint32_t)o[3] << 16);
-        r.z = o[4] | ((uint32_t)o[5] << 16); r.w = o[6] | ((uint32_t)o[7] << 16);
-        *reinterpret_cast<uint4*>(out + ((((long long)n * Ho + y) * Wo + x) * C) + g * 8) = r;
+        *reinterpret_cast<uint4*>(d) = pack8(o);
     }
 }
 
-// L2Norm (net_s3fd.py:6-19): x / (sqrt(sum_c x^2) + 1e-10) * weight[c]; one warp per pixel
+// L2Norm (net_s3fd.py:6-19): x / (sqrt(sum_c x^2) + 1e-10) * weight[c]; one warp per pixel.  Split operands: x = hi + lo
+// (exact in fp32), y is stored as to16(y) and to16(y - hi).
 template <bool kBF16>
-__global__ void chan_l2norm_kernel(const uint16_t* in, uint16_t* out, const float* weight, long long pixels, int C) {
+__global__ void chan_l2norm_kernel(const uint16_t* in, uint16_t* out, const float* weight, long long pixels, int C, int Cs,
+                                   int lo_off) {
     const long long pix = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (pix >= pixels) return;
-    const uint16_t* p = in + pix * C;
+    const uint16_t* p = in + pix * Cs;
+    uint16_t* q = out + pix * Cs;
+    auto val = [&](int c) { return lo_off > 0 ? from16<kBF16>(p[c]) + from16<kBF16>(p[c + lo_off]) : from16<kBF16>(p[c]); };
     float s = 0.0f;
-    for (int c = lane; c < C; c += 32) { const float v = from16<kBF16>(p[c]); s = fmaf(v, v, s); }
+    for (int c = lane; c < C; c += 32) { const float v = val(c); s = fmaf(v, v, s); }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const float inv = 1.0f / (sqrtf(s) + 1e-10f);
-    for (int c = lane; c < C; c += 32) out[pix * C + c] = to16<kBF16>(from16<kBF16>(p[c]) * inv * __ldg(weight + c));
+    for (int c = lane; c < C; c += 32) {
+        const float y = val(c) * inv * __ldg(weight + c);
+        const uint16_t h = to16<kBF16>(y);
+        q[c] = h;
+        if (lo_off > 0) q[c + lo_off] = to16<kBF16>(y - from16<kBF16>(h));
+    }
 }
 
 // mbox head (fp32 NHWC, 16-channel pitch) -> the module's NCHW fp32 output; maxout: cls1 = [max(c0,c1,c2), c3] (net_s3fd.py:123-126)

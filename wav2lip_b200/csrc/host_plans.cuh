@@ -277,12 +277,16 @@ static int build_s3fd_plan(w2l_ctx* ctx, Plan* pl) {
         pl->layer_out[li] = *out;
         return W2L_OK;
     };
+    // pools and L2Norms are exported by w2l_debug_layer_output after the 31 conv layers: pool k at 31 + k, norm i at 36 + i
+    int npool = 0;
     auto pool = [&](const Act& in, Act* out) -> int {
         CKR(plan_act(pl, out, N, in.H / 2, in.W / 2, in.C));
         Op op;
         op.type = OP_MAXPOOL; op.name = "max_pool2d";
         op.sp_in = in.base; op.sp_out = out->base; op.sp_N = N; op.sp_H = in.H; op.sp_W = in.W; op.sp_C = in.C;
+        op.aux_pitch = in.Cs; op.aux_lo = in.lo_off;   // the output has the input's layout
         pl->ops.push_back(op);
+        pl->layer_out[(int)sp.layers.size() + npool++] = *out;
         return W2L_OK;
     };
     Act a, b, taps[6];
@@ -302,7 +306,9 @@ static int build_s3fd_plan(w2l_ctx* ctx, Plan* pl) {
             op.type = OP_CHAN_L2NORM; op.name = "L2Norm";
             op.sp_in = taps[i].base; op.sp_out = f.base; op.sp_w = ctx->s3fd_l2w[i];
             op.sp_N = N; op.sp_H = f.H; op.sp_W = f.W; op.sp_C = f.C;
+            op.aux_pitch = f.Cs; op.aux_lo = f.lo_off;
             pl->ops.push_back(op);
+            pl->layer_out[(int)sp.layers.size() + 5 + i] = f;
         }
         for (int h = 0; h < 2; ++h) {
             const int li = 19 + 2 * i + h;
@@ -460,15 +466,15 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
             case OP_MAXPOOL: {
                 const long long total = (long long)op.sp_N * (op.sp_H / 2) * (op.sp_W / 2) * (op.sp_C / 8);
                 const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-                if (ctx->bf16) maxpool2_kernel<true><<<blocks, 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_N, op.sp_H, op.sp_W, op.sp_C);
-                else maxpool2_kernel<false><<<blocks, 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_N, op.sp_H, op.sp_W, op.sp_C);
+                if (ctx->bf16) maxpool2_kernel<true><<<blocks, 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_N, op.sp_H, op.sp_W, op.sp_C, op.aux_pitch, op.aux_lo);
+                else maxpool2_kernel<false><<<blocks, 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_N, op.sp_H, op.sp_W, op.sp_C, op.aux_pitch, op.aux_lo);
                 ctx->launches++;
                 break;
             }
             case OP_CHAN_L2NORM: {
                 const long long pixels = (long long)op.sp_N * op.sp_H * op.sp_W;
-                if (ctx->bf16) chan_l2norm_kernel<true><<<(unsigned)((pixels + 7) / 8), 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_w, pixels, op.sp_C);
-                else chan_l2norm_kernel<false><<<(unsigned)((pixels + 7) / 8), 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_w, pixels, op.sp_C);
+                if (ctx->bf16) chan_l2norm_kernel<true><<<(unsigned)((pixels + 7) / 8), 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_w, pixels, op.sp_C, op.aux_pitch, op.aux_lo);
+                else chan_l2norm_kernel<false><<<(unsigned)((pixels + 7) / 8), 256, 0, st>>>(op.sp_in, op.sp_out, op.sp_w, pixels, op.sp_C, op.aux_pitch, op.aux_lo);
                 ctx->launches++;
                 break;
             }

@@ -140,7 +140,7 @@ struct Op {
     const void* aux_in = nullptr;
     int aux_rows = 0, aux_dim = 0;
     int aux_out = 0;  // which caller output
-    int aux_pitch = 0, aux_lo = 0;
+    int aux_pitch = 0, aux_lo = 0;  // pixel pitch and lo-plane offset of aux_in (also of the S3FD max-pool / L2Norm buffers)
     // S3FD: max-pool / channel L2Norm / head export
     const uint16_t* sp_in = nullptr; uint16_t* sp_out = nullptr; const float* sp_f32 = nullptr; const float* sp_w = nullptr;
     int sp_N = 0, sp_H = 0, sp_W = 0, sp_C = 0, sp_Cout = 0, sp_maxout = 0;
