@@ -33,22 +33,12 @@ static void build_mel_basis(std::vector<float>* dense) {
 }
 
 static int init_mel_tables(w2l_ctx* ctx) {
-    std::vector<double2> tw(MEL_TW_TOTAL);
+    std::vector<double2> tw(MEL_BINS);  // exp(-2 pi i m / 800), m = 0..400
     const long double kTwoPi = 2.0L * 3.141592653589793238462643383279502884L;
-    for (int m = 0; m <= 400; ++m) {  // post-pass / window table: exp(-2 pi i m / 800)
+    for (int m = 0; m < MEL_BINS; ++m) {
         const long double a = -kTwoPi * m / MEL_NFFT;
-        tw[MEL_TW_POST + m] = make_double2((double)cosl(a), (double)sinl(a));
+        tw[m] = make_double2((double)cosl(a), (double)sinl(a));
     }
-    auto fill_pass = [&](int base, int R, int Ns) {  // T[r-1][k] = exp(-2 pi i r k / (Ns R))
-        for (int r = 1; r < R; ++r)
-            for (int k = 0; k < Ns; ++k) {
-                const long double a = -kTwoPi * (long double)(r * k) / (long double)(Ns * R);
-                tw[base + (r - 1) * Ns + k] = make_double2((double)cosl(a), (double)sinl(a));
-            }
-    };
-    fill_pass(MEL_TW_P2, 5, 5);
-    fill_pass(MEL_TW_P3, 4, 25);
-    fill_pass(MEL_TW_P4, 4, 100);
     std::vector<float> dense;
     build_mel_basis(&dense);
     std::vector<float> vals;
@@ -74,7 +64,6 @@ static int init_mel_tables(w2l_ctx* ctx) {
     CK(cudaMemcpy(ctx->mel_bstart, start.data(), MEL_BANDS * 4, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->mel_blen, len.data(), MEL_BANDS * 4, cudaMemcpyHostToDevice));
     CK(cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMelSmemBytes));
-    CK(cudaFuncSetAttribute(mel_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, kMel2SmemBytes));
     return W2L_OK;
 }
 

@@ -189,7 +189,6 @@ struct w2l_ctx {
     bool use_ctfused = true;  // W2L_DISABLE_CTFUSED=1
     bool use_fold = true;   // W2L_DISABLE_FOLD=1 / driver rejects overlapping-stride tensor maps
     bool use_pdl = true;      // W2L_DISABLE_PDL=1
-    bool use_mel_v2 = true;    // W2L_DISABLE_MELV2=1
     NetW nets[4];
     float* s3fd_l2w[3] = {nullptr, nullptr, nullptr};   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)
     std::map<std::string, std::unique_ptr<Plan>> plans;

@@ -10,11 +10,21 @@
 // float64 matters: with a loud tone in the frame, a float32 FFT's noise floor (-144 dB re peak) reaches
 // the mel bands near the 1e-5 clipping floor and breaks the 1e-4 tolerance; the H100 has the FP64 rate.
 //
-// Work split: a block owns MEL_FPB consecutive frames (so the (80, F) row-major output is written in
-// 16-byte runs), MEL_TPF threads per frame. The real 800-point FFT is a 400-point complex Stockham FFT
-// (radix 5,5,4,4 — 800 = 2^5 5^2 is not a power of two and zero-padding would change the result) in
-// shared memory, followed by the even/odd split post-pass; the mel product uses the filterbank's
-// sparsity (739 non-zeros, <= 27 per band) straight from the magnitudes in shared memory.
+// Work split: a block owns MEL_FPB consecutive frames (so the (80, F) row-major output is written in runs of
+// MEL_FPB floats). The real 800-point FFT is the 400-point complex FFT of the even/odd-packed frame followed by
+// the real-FFT split X[k] = E[k] + W800^k O[k] (800 = 2^5 5^2 is not a power of two, and zero-padding would
+// change the result). 400 = 25 x 16 is split Cooley-Tukey style across threads:
+//   step 1  (25 threads per frame, thread = n1): the 16 packed samples z[n1 + 25 n2] are gathered straight from
+//           HBM/L1 (coalesced across n1), pre-emphasised, windowed (periodic Hann from the cos table) and transformed
+//           by a 16-point FFT (4 x 4) in registers; the result is multiplied by W400^(n1 k2) and written to shared
+//           memory, the one exchange between the two steps;
+//   step 3  (16 threads per frame, thread = k2): 25-point FFT (5 x 5) in registers over n1, then the real-FFT
+//           split, whose partner Z[400 - k] lives in thread 16 - k2 of the same 16-lane group: warp shuffles,
+//           no second exchange; |X| goes to shared memory as fp32.
+// The twiddles inside the small FFTs are compile-time constants (mel_consts.h). The FFT lives in registers because
+// a shared-memory round trip of the float64 data per radix pass would make the kernel shared-memory bound; with one
+// exchange (~18 KB of shared-memory traffic per frame) it is bound by the FP64 pipe instead. The mel product uses
+// the filterbank's sparsity (739 non-zeros, <= 27 per band) straight from the magnitudes in shared memory.
 #pragma once
 
 #include <stdint.h>
@@ -23,20 +33,20 @@
 
 namespace w2l {
 
-constexpr int MEL_FPB = 4;
-constexpr int MEL_TPF = 128;
+constexpr int MEL_FPB = 5;        // frames per block: 125 of 128 threads busy in step 1, 80 in step 3
+constexpr int MEL_THREADS = 128;
 constexpr int MEL_NFFT = 800;
 constexpr int MEL_HOP = 200;
 constexpr int MEL_BINS = 401;
 constexpr int MEL_BANDS = 80;
+constexpr int kMelSmemBytes = 404 * 16 + MEL_FPB * 400 * 16 + MEL_FPB * 404 * 4 + MEL_BANDS * MEL_FPB * 4;
 
 struct MelParams {
     const float* wav;
     long long L;
     float* mel;          // (80, F) row-major
     long long F;
-    const double2* tw;   // [0,401): exp(-2 pi i m / 800) (window + real-FFT post pass); [401, 401+395): per-pass twiddles
-                         // T[r][k] = exp(-2 pi i r k / (Ns R)), r-major so that a warp reads consecutive k (no bank conflicts)
+    const double2* tw;   // [0,401): exp(-2 pi i m / 800) (Hann window, W400 twiddles of step 1, real-FFT split)
     const float* bvals;  // packed non-zero filterbank weights
     const int* boff;     // [80] offset into bvals
     const int* bstart;   // [80] first FFT bin of the band
@@ -81,147 +91,24 @@ __device__ __forceinline__ void butterfly<5>(double2* v) {
     v[3] = make_double2(t2.x - u2.y, t2.y + u2.x);
 }
 
-// Twiddle table layout in shared memory (double2 units)
-constexpr int MEL_TW_POST = 0;                 // 401 entries
-constexpr int MEL_TW_P2 = 401;                 // radix 5, Ns = 5  : T[r-1][k], r = 1..4, k < 5    (20)
-constexpr int MEL_TW_P3 = MEL_TW_P2 + 20;      // radix 4, Ns = 25 : T[r-1][k], r = 1..3, k < 25   (75)
-constexpr int MEL_TW_P4 = MEL_TW_P3 + 75;      // radix 4, Ns = 100: T[r-1][k], r = 1..3, k < 100  (300)
-constexpr int MEL_TW_TOTAL = MEL_TW_P4 + 300;  // 796
-
-// One Stockham pass of a 400-point FFT: radix R, Ns = product of the radices already applied.
-// tw_pass = this pass's r-major twiddle table (nullptr for the first pass, whose twiddles are all 1).
-template <int R>
-__device__ __forceinline__ void fft400_pass(const double2* in, double2* out, int j, int Ns, const double2* tw_pass) {
-    const int k = j % Ns;
-    double2 v[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        v[r] = in[j + r * (400 / R)];
-        if (r > 0 && tw_pass != nullptr) v[r] = cmul(v[r], tw_pass[(r - 1) * Ns + k]);
-    }
-    butterfly<R>(v);
-    const int j0 = (j / Ns) * Ns * R + k;
-#pragma unroll
-    for (int r = 0; r < R; ++r) out[j0 + r * Ns] = v[r];
-}
-
-__global__ void __launch_bounds__(MEL_FPB* MEL_TPF) mel_kernel(const MelParams p) {
-    extern __shared__ uint8_t mel_smem[];
-    double2* tw = reinterpret_cast<double2*>(mel_smem);                       // [MEL_TW_TOTAL]
-    double2* bufs = tw + MEL_TW_TOTAL;                                        // [FPB][2][400]
-    float* mags = reinterpret_cast<float*>(bufs + MEL_FPB * 2 * 400);         // [FPB][404]
-    float* outs = mags + MEL_FPB * 404;                                       // [80][FPB]
-
-    const int f = threadIdx.x / MEL_TPF;
-    const int tid = threadIdx.x % MEL_TPF;
-    const long long t = (long long)blockIdx.x * MEL_FPB + f;
-    const bool live = t < p.F;
-
-    for (int i = threadIdx.x; i < MEL_TW_TOTAL; i += blockDim.x) tw[i] = p.tw[i];
-    __syncthreads();
-
-    double2* b0 = bufs + f * 800;
-    double2* b1 = b0 + 400;
-    float* mag = mags + f * 404;
-
-    // ---- frame gather: reflect pad of the PRE-EMPHASISED signal, Hann window, even/odd packing ----
-    if (live) {
-        for (int i = tid; i < 400; i += MEL_TPF) {
-            double s[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int n = 2 * i + e;
-                long long j = t * MEL_HOP + n - MEL_NFFT / 2;
-                // np.pad(mode="reflect") index folding; clips shorter than n_fft/2 reflect more than once
-                while (j < 0 || j >= p.L) j = j < 0 ? -j : 2 * (p.L - 1) - j;
-                const double x0 = (double)__ldg(p.wav + j);
-                const double y = (j > 0) ? x0 + (-0.97) * (double)__ldg(p.wav + j - 1) : x0;
-                const double w = 0.5 - 0.5 * tw[n <= 400 ? n : MEL_NFFT - n].x;  // periodic Hann: 0.5 - 0.5 cos(2 pi n / 800)
-                s[e] = w * y;
-            }
-            b0[i] = make_double2(s[0], s[1]);
-        }
-    }
-    __syncthreads();
-    if (live && tid < 80) fft400_pass<5>(b0, b1, tid, 1, nullptr);
-    __syncthreads();
-    if (live && tid < 80) fft400_pass<5>(b1, b0, tid, 5, tw + MEL_TW_P2);
-    __syncthreads();
-    if (live && tid < 100) fft400_pass<4>(b0, b1, tid, 25, tw + MEL_TW_P3);
-    __syncthreads();
-    if (live && tid < 100) fft400_pass<4>(b1, b0, tid, 100, tw + MEL_TW_P4);
-    __syncthreads();
-    // ---- real-FFT post pass: X[k] = E[k] + W800^k O[k]; round to complex64; magnitude in fp32 ----
-    if (live) {
-        for (int k = tid; k < MEL_BINS; k += MEL_TPF) {
-            const double2 zk = b0[k % 400];
-            const double2 zm = b0[(400 - k) % 400];
-            const double2 e = make_double2(0.5 * (zk.x + zm.x), 0.5 * (zk.y - zm.y));
-            const double2 d = make_double2(0.5 * (zk.x - zm.x), 0.5 * (zk.y + zm.y));
-            const double2 o = make_double2(d.y, -d.x);  // -i d
-            const double2 x = cadd(e, cmul(tw[k], o));
-            const float re = (float)x.x, im = (float)x.y;  // complex64 store of librosa.stft
-            mag[k] = (float)sqrt((double)re * (double)re + (double)im * (double)im);
-        }
-    }
-    __syncthreads();
-    // ---- sparse mel product + dB + normalise/clip, all fp32 as NumPy does on float32 arrays ----
-    if (live && tid < MEL_BANDS) {
-        const int off = p.boff[tid], st = p.bstart[tid], len = p.blen[tid];
-        float s = 0.0f;
-        for (int j = 0; j < len; ++j) s = fmaf(__ldg(p.bvals + off + j), mag[st + j], s);
-        float db = 20.0f * log10f(fmaxf(1e-5f, s)) - 20.0f;
-        float v = 8.0f * ((db + 100.0f) / 100.0f) - 4.0f;
-        v = fminf(fmaxf(v, -4.0f), 4.0f);
-        outs[tid * MEL_FPB + f] = v;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < MEL_BANDS * MEL_FPB; i += blockDim.x) {
-        const int m = i / MEL_FPB, ff = i % MEL_FPB;
-        const long long tt = (long long)blockIdx.x * MEL_FPB + ff;
-        if (tt < p.F) p.mel[(long long)m * p.F + tt] = outs[i];
-    }
-}
-
-constexpr int kMelSmemBytes = MEL_TW_TOTAL * 16 + MEL_FPB * 800 * 16 + MEL_FPB * 404 * 4 + MEL_BANDS * MEL_FPB * 4;
-
-// ------------------------------------------------------------------------------------------------
-// mel_kernel_v2 — the same arithmetic with the 400-point FFT held in REGISTERS (round 2).
-//
-// The first version round-tripped double2 data through shared memory on every Stockham pass and was shared-memory bound
-// (ncu: l1tex 85 %, 0.026 of the HBM roof).  Here 400 = 25 x 16 is split Cooley-Tukey style across threads:
-//   step 1  (25 threads per frame, thread = n1): the 16 packed samples z[n1 + 25 n2] are gathered straight from HBM/L1
-//           (coalesced across n1), pre-emphasised, windowed (Hann from two table values per thread and compile-time
-//           (cos, sin)(n2 pi/8) constants) and transformed by a 16-point FFT (4 x 4) entirely in registers; the result is
-//           multiplied by W400^(n1 k2) (a 15-step recurrence from one table value) and written ONCE to shared memory;
-//   step 3  (16 threads per frame, thread = k2): 25-point FFT (5 x 5) in registers over n1, then the real-FFT split
-//           X[k] = E[k] + W800^k O[k], whose partner Z[400 - k] lives in thread 16 - k2 of the same 16-lane group:
-//           warp shuffles, no second shared-memory pass; |X| goes to shared memory as fp32 for the sparse mel product.
-// Shared-memory traffic per frame drops from ~70 KB to ~18 KB; all twiddles inside the small FFTs are compile-time
-// constants (mel_consts.h).  Same dtypes as before: float64 up to the complex64 rounding of the spectrum, fp32 after.
-// ------------------------------------------------------------------------------------------------
-constexpr int MEL2_FPB = 5;        // frames per block: 125 of 128 threads busy in step 1, 80 in step 3
-constexpr int MEL2_THREADS = 128;
-constexpr int kMel2SmemBytes = 404 * 16 + MEL2_FPB * 400 * 16 + MEL2_FPB * 404 * 4 + MEL_BANDS * MEL2_FPB * 4;
-
 __device__ __forceinline__ double2 shfl_d2(double2 v, int src_lane) {
     return make_double2(__shfl_sync(0xffffffffu, v.x, src_lane, 16), __shfl_sync(0xffffffffu, v.y, src_lane, 16));
 }
 
-__global__ void __launch_bounds__(MEL2_THREADS, 4) mel_kernel_v2(const MelParams p) {
+__global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) {
     extern __shared__ uint8_t mel_smem[];
     double2* tw = reinterpret_cast<double2*>(mel_smem);                 // [401] exp(-2 pi i m / 800)  (+3 pad)
     double2* ybuf = tw + 404;                                            // [FPB][16][25]
-    float* mags = reinterpret_cast<float*>(ybuf + MEL2_FPB * 400);       // [FPB][404]
-    float* outs = mags + MEL2_FPB * 404;                                 // [80][FPB]
+    float* mags = reinterpret_cast<float*>(ybuf + MEL_FPB * 400);        // [FPB][404]
+    float* outs = mags + MEL_FPB * 404;                                  // [80][FPB]
     const int tid = threadIdx.x;
-    for (int i = tid; i < 401; i += MEL2_THREADS) tw[i] = p.tw[i];
+    for (int i = tid; i < 401; i += MEL_THREADS) tw[i] = p.tw[i];
     __syncthreads();
 
     // ---------------- step 1: thread = (frame f, n1) ----------------
-    if (tid < MEL2_FPB * 25) {
+    if (tid < MEL_FPB * 25) {
         const int f = tid / 25, n1 = tid % 25;
-        const long long t = (long long)blockIdx.x * MEL2_FPB + f;
+        const long long t = (long long)blockIdx.x * MEL_FPB + f;
         if (t < p.F) {
             double2 v[16];
             const long long base = t * MEL_HOP - MEL_NFFT / 2 + 2 * n1;
@@ -283,8 +170,8 @@ __global__ void __launch_bounds__(MEL2_THREADS, 4) mel_kernel_v2(const MelParams
     // ---------------- step 3: thread = (frame f, k2), whole warps so that the shuffles below are convergent ----------------
     if (tid < 96) {
         const int f = tid >> 4, k2 = tid & 15;
-        const long long t = (long long)blockIdx.x * MEL2_FPB + f;
-        const bool live = f < MEL2_FPB && t < p.F;
+        const long long t = (long long)blockIdx.x * MEL_FPB + f;
+        const bool live = f < MEL_FPB && t < p.F;
         double2 y[25];
 #pragma unroll
         for (int n1 = 0; n1 < 25; ++n1) y[n1] = live ? ybuf[f * 400 + k2 * 25 + n1] : make_double2(0.0, 0.0);
@@ -328,9 +215,9 @@ __global__ void __launch_bounds__(MEL2_THREADS, 4) mel_kernel_v2(const MelParams
     }
     __syncthreads();
     // ---------------- sparse mel product + dB + normalise / clip, fp32 as NumPy does on float32 arrays ----------------
-    for (int i = tid; i < MEL_BANDS * MEL2_FPB; i += MEL2_THREADS) {
+    for (int i = tid; i < MEL_BANDS * MEL_FPB; i += MEL_THREADS) {
         const int f = i / MEL_BANDS, m = i % MEL_BANDS;
-        const long long t = (long long)blockIdx.x * MEL2_FPB + f;
+        const long long t = (long long)blockIdx.x * MEL_FPB + f;
         if (t >= p.F) continue;
         const float* mag = mags + f * 404;
         const int off = p.boff[m], st = p.bstart[m], len = p.blen[m];
@@ -339,12 +226,12 @@ __global__ void __launch_bounds__(MEL2_THREADS, 4) mel_kernel_v2(const MelParams
         const float db = 20.0f * log10f(fmaxf(1e-5f, s)) - 20.0f;
         float v = 8.0f * ((db + 100.0f) / 100.0f) - 4.0f;
         v = fminf(fmaxf(v, -4.0f), 4.0f);
-        outs[m * MEL2_FPB + f] = v;
+        outs[m * MEL_FPB + f] = v;
     }
     __syncthreads();
-    for (int i = tid; i < MEL_BANDS * MEL2_FPB; i += MEL2_THREADS) {
-        const int m = i / MEL2_FPB, ff = i % MEL2_FPB;
-        const long long tt = (long long)blockIdx.x * MEL2_FPB + ff;
+    for (int i = tid; i < MEL_BANDS * MEL_FPB; i += MEL_THREADS) {
+        const int m = i / MEL_FPB, ff = i % MEL_FPB;
+        const long long tt = (long long)blockIdx.x * MEL_FPB + ff;
         if (tt < p.F) p.mel[(long long)m * p.F + tt] = outs[i];
     }
 }

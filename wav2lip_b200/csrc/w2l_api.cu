@@ -120,7 +120,6 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
         ctx->use_ctfused = enabled("W2L_DISABLE_CTFUSED");
         ctx->use_side = enabled("W2L_DISABLE_SIDESTREAM");
         ctx->use_pdl = enabled("W2L_DISABLE_PDL");
-        ctx->use_mel_v2 = enabled("W2L_DISABLE_MELV2");
         if (ctx->x2) {  // the split-operand mode runs on the generic kernel with the direct epilogue only
             ctx->use_patch = ctx->use_fold = ctx->use_fold_s2 = ctx->use_ctfused = ctx->use_tma_epi = false;
         }
@@ -290,11 +289,8 @@ static int host_submit(w2l_ctx* ctx, int B, int T, const void* mel_h, size_t mel
     return W2L_OK;
 }
 
-static int host_chunks(int B) {
-    int n = B >= 64 ? 2 : 1;  // fewer, larger chunks: small batches run the low-resolution layers inefficiently
-    if (const char* ev = getenv("W2L_HOST_CHUNKS")) n = std::max(1, std::min(atoi(ev), B));
-    return n;
-}
+// fewer, larger chunks: small batches run the low-resolution layers inefficiently
+static int host_chunks(int B) { return B >= 64 ? 2 : 1; }
 
 int w2l_generator_forward_host(w2l_ctx* ctx, const float* mel_h, const float* face_h, float* out_h, int B, int T) {
     if (!ctx || !mel_h || !face_h || !out_h) return fail(W2L_EINVAL, "null argument");
@@ -799,13 +795,8 @@ int w2l_melspectrogram(w2l_ctx* ctx, const float* wav, int64_t n_samples, float*
     MelParams p;
     p.wav = wav; p.L = n_samples; p.mel = mel; p.F = w2l_mel_num_frames(n_samples);
     p.tw = ctx->mel_tw; p.bvals = ctx->mel_bvals; p.boff = ctx->mel_boff; p.bstart = ctx->mel_bstart; p.blen = ctx->mel_blen;
-    if (ctx->use_mel_v2) {   // FFT in registers (mel.cuh, round 2); W2L_DISABLE_MELV2=1 selects the shared-memory version
-        const long long blocks = (p.F + MEL2_FPB - 1) / MEL2_FPB;
-        mel_kernel_v2<<<(unsigned)blocks, MEL2_THREADS, kMel2SmemBytes, (cudaStream_t)stream>>>(p);
-    } else {
-        const long long blocks = (p.F + MEL_FPB - 1) / MEL_FPB;
-        mel_kernel<<<(unsigned)blocks, MEL_FPB * MEL_TPF, kMelSmemBytes, (cudaStream_t)stream>>>(p);
-    }
+    const long long blocks = (p.F + MEL_FPB - 1) / MEL_FPB;
+    mel_kernel<<<(unsigned)blocks, MEL_THREADS, kMelSmemBytes, (cudaStream_t)stream>>>(p);
     ctx->launches++;
     CK(cudaGetLastError());
     return W2L_OK;
