@@ -416,7 +416,8 @@ int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* o
 /* ---- instrumentation ---- */
 /* kernels launched by this library since the context was created (all streams) */
 int64_t w2l_launch_count(const w2l_ctx* ctx);
-/* bytes of device memory currently held by the context (weights + activation arenas) */
+/* bytes of device memory the context holds: weights, inference and training plans, Adam moments, staging and scratch
+ * buffers, mel tables — every block it has allocated and not yet released */
 int64_t w2l_device_bytes(const w2l_ctx* ctx);
 /* Time the conv kernels of the last-built plan of `net` individually: runs every launch `iters`
  * times with CUDA events on `stream`, the L2 flushed before each timed launch (cold cache, as in the step), and writes

@@ -1,4 +1,4 @@
-// host_mel_tables.h — host-side tables of the mel kernel (twiddles, sparse Slaney filterbank), staging buffers, DeviceGuard.
+// host_mel_tables.h — host-side tables of the mel kernel (twiddles, sparse Slaney filterbank).
 // Part of the single translation unit w2l_api.cu (included there, in this order).
 #pragma once
 
@@ -52,12 +52,11 @@ static int init_mel_tables(w2l_ctx* ctx) {
         len[i] = a < 0 ? 0 : b - a + 1;
         for (int k = 0; k < len[i]; ++k) vals.push_back(dense[(size_t)i * MEL_BINS + start[i] + k]);
     }
-    void* p;
-    CKR(dev_alloc(&p, tw.size() * sizeof(double2))); ctx->mel_tw = (double2*)p;
-    CKR(dev_alloc(&p, vals.size() * 4)); ctx->mel_bvals = (float*)p;
-    CKR(dev_alloc(&p, MEL_BANDS * 4)); ctx->mel_boff = (int*)p;
-    CKR(dev_alloc(&p, MEL_BANDS * 4)); ctx->mel_bstart = (int*)p;
-    CKR(dev_alloc(&p, MEL_BANDS * 4)); ctx->mel_blen = (int*)p;
+    CKR(ctx->mel_tw.grow(ctx, tw.size() * sizeof(double2)));
+    CKR(ctx->mel_bvals.grow(ctx, vals.size() * 4));
+    CKR(ctx->mel_boff.grow(ctx, MEL_BANDS * 4));
+    CKR(ctx->mel_bstart.grow(ctx, MEL_BANDS * 4));
+    CKR(ctx->mel_blen.grow(ctx, MEL_BANDS * 4));
     CK(cudaMemcpy(ctx->mel_tw, tw.data(), tw.size() * sizeof(double2), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->mel_bvals, vals.data(), vals.size() * 4, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->mel_boff, off.data(), MEL_BANDS * 4, cudaMemcpyHostToDevice));
@@ -66,18 +65,3 @@ static int init_mel_tables(w2l_ctx* ctx) {
     CK(cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMelSmemBytes));
     return W2L_OK;
 }
-
-static int ensure_stage(w2l_ctx* ctx, int i, size_t bytes) {
-    if (ctx->stage_bytes[i] >= bytes) return W2L_OK;
-    if (ctx->stage[i]) cudaFree(ctx->stage[i]);
-    ctx->stage[i] = nullptr; ctx->stage_bytes[i] = 0;
-    CKR(dev_alloc(&ctx->stage[i], bytes));
-    ctx->stage_bytes[i] = bytes;
-    return W2L_OK;
-}
-
-struct DeviceGuard {
-    int prev = -1;
-    explicit DeviceGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
-    ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-};

@@ -348,14 +348,13 @@ static int ensure_s3fd_detect(w2l_ctx* ctx, Plan* pl) {
     p.Lpad = 1;
     while (p.Lpad < L) p.Lpad <<= 1;
     p.nchunk = (L + kSelChunk - 1) / kSelChunk;
-    void* q;
-    CKR(plan_alloc(pl, &q, (size_t)B * p.nchunk * 4)); p.chunk_count = (int*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * 4)); p.ncand = (int*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * L * 16)); p.cbox = (float4*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * L * 4)); p.cloc = (int*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * p.Lpad * 8)); p.keys = (uint64_t*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * L)); p.sup = (uint8_t*)q;
-    CKR(plan_alloc(pl, &q, (size_t)B * 4)); p.path = (int*)q;
+    CKR(plan_alloc(pl, &p.chunk_count, (size_t)B * p.nchunk * 4));
+    CKR(plan_alloc(pl, &p.ncand, (size_t)B * 4));
+    CKR(plan_alloc(pl, &p.cbox, (size_t)B * L * 16));
+    CKR(plan_alloc(pl, &p.cloc, (size_t)B * L * 4));
+    CKR(plan_alloc(pl, &p.keys, (size_t)B * p.Lpad * 8));
+    CKR(plan_alloc(pl, &p.sup, (size_t)B * L));
+    CKR(plan_alloc(pl, &p.path, (size_t)B * 4));
     CK(cudaFuncSetAttribute(s3fd_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kNmsSmemBytes));
     pl->det = std::move(dw);
     return W2L_OK;
@@ -388,10 +387,9 @@ static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, 
         if (count < 6) break;
         CK(cudaDeviceSynchronize());  // the plan's buffers may still be in use by queued launches
         if (ctx->last_plan[net] == lru->second.get()) ctx->last_plan[net] = nullptr;
-        free_plan(lru->second.get());
         ctx->plans.erase(lru);
     }
-    std::unique_ptr<Plan> pl(new Plan());
+    std::unique_ptr<Plan> pl(new Plan(ctx));
     pl->net = net; pl->B = B; pl->T = T; pl->H = H; pl->W = W;
     pl->x2 = ctx->x2;
     pl->N = (net == W2L_NET_SYNCNET) ? B : (T > 0 ? B * T : B);
@@ -400,7 +398,7 @@ static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, 
     else if (net == W2L_NET_SYNCNET) r = build_syncnet_plan(ctx, pl.get());
     else if (net == W2L_NET_S3FD) r = build_s3fd_plan(ctx, pl.get());
     else r = build_disc_plan(ctx, pl.get());
-    if (r != W2L_OK) { free_plan(pl.get()); return r; }
+    CKR(r);
     pl->last_used = ++ctx->plan_clock;
     *out = pl.get();
     ctx->plans[key] = std::move(pl);

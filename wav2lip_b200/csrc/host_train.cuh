@@ -52,11 +52,12 @@ struct TBlock {
 };
 
 struct TrainPlan {
+    explicit TrainPlan(w2l_ctx* ctx) : pl(ctx) {}
     int net = 0, B = 0, T = 0, N = 0;
     Plan pl;                       // op storage + allocations
     NetW wf, wd;                   // forward / dgrad weight slabs (16-bit), repacked every step
     RepackLog repack;              // ... by these launches
-    PackParams* pack_dev = nullptr; int *pack_blk_job = nullptr, *pack_blk_first = nullptr; int pack_blocks = 0;   // one-launch repack
+    DevMem<PackParams> pack_dev; DevMem<int> pack_blk_job, pack_blk_first; int pack_blocks = 0;   // one-launch repack
     std::vector<TBlock> blocks;    // forward order
     std::vector<size_t> ingest;    // indices of the ingest ops
     // generator
@@ -76,7 +77,7 @@ struct TrainPlan {
 
 // Adam moments of one net's bound tensors that have a gradient, in the order of the name map (alphabetical): names[i] owns
 // host[i]; step is the count the bias correction uses (torch.optim.Adam's state['step'])
-struct AdamSlot { std::vector<std::string> names; std::vector<float*> m, v; std::vector<AdamTensor> host; AdamTensor* dev = nullptr; long long step = 0; };
+struct AdamSlot { std::vector<std::string> names; std::vector<DevMem<>> moments; std::vector<AdamTensor> host; DevMem<AdamTensor> dev; long long step = 0; };
 
 // NCCL entry points resolved at run time from the libnccl.so.2 that torch already loaded (no link-time dependency)
 typedef int (*NcclGetUniqueIdFn)(void*);
@@ -93,58 +94,29 @@ struct TrainState {
     TrainPlan* last[3] = {nullptr, nullptr, nullptr};
     AdamSlot adam[3];
     // losses of the fused steps
-    float* loss_dev = nullptr;     // [8]
-    float *a_emb = nullptr, *v_emb = nullptr, *da = nullptr, *dv = nullptr; int emb_cap = 0;
-    float* g_buf = nullptr; float* dg_buf = nullptr; size_t g_cap = 0;
-    float *prob = nullptr, *dprob = nullptr; int prob_cap = 0;   // disc probabilities on g | gt (2N), their gradients (3N)
+    DevMem<float> loss_dev;        // [8]
+    DevMem<float> a_emb, v_emb, da, dv;
+    DevMem<float> g_buf, dg_buf;
+    DevMem<float> prob, dprob;     // disc probabilities on g | gt (2N), their gradients (3N)
     // data-parallel gradient all-reduce
     void* nccl_lib = nullptr; void* comm = nullptr; int rank = 0, world = 1;
     NcclAllReduceFn all_reduce = nullptr; NcclCommDestroyFn comm_destroy = nullptr; NcclGetErrorStringFn err_string = nullptr;
-    cudaStream_t s_comm = nullptr; cudaEvent_t ev_bucket = nullptr, ev_comm = nullptr;
+    Stream s_comm; Event ev_bucket, ev_comm;
     double last_allreduce_bytes = 0;
     // the weight-gradient GEMMs are leaves of the backward graph: they run on a side stream beside the dgrad chain, so that
     // they fill the SMs the chain's partial rounds (and, at small batches, its latency-bound launches) leave idle
-    cudaStream_t s_wg = nullptr; cudaEvent_t ev_dz = nullptr, ev_wg = nullptr, ev_wgb = nullptr;
+    Stream s_wg; Event ev_dz, ev_wg, ev_wgb;
     // the audio encoder (small, latency-bound launches) runs beside the face encoder, forward and backward
-    cudaStream_t s_aux = nullptr; cudaEvent_t ev_aux_fork = nullptr, ev_aux_join = nullptr;
+    Stream s_aux; Event ev_aux_fork, ev_aux_join;
     // the discriminator's step of the hq iteration (its two backward passes, all-reduce, Adam) beside the generator's backward
-    cudaStream_t s_disc = nullptr; cudaEvent_t ev_disc_fork = nullptr, ev_disc_join = nullptr;
+    Stream s_disc; Event ev_disc_fork, ev_disc_join;
     std::vector<w2l_train_block_info> last_block_info;   // the block of the last w2l_conv_block_train (its plan is freed)
+    ~TrainState() { if (comm && comm_destroy) comm_destroy(comm); }   // before s_comm goes
 };
 
 static TrainState* train_state(w2l_ctx* ctx) {
-    if (!ctx->train) ctx->train = new TrainState();
-    return ctx->train;
-}
-
-static void free_train_plan(TrainPlan* tp) {
-    free_plan(&tp->pl);
-    for (auto& lw : tp->wf.layers) free_layer(lw);
-    for (auto& lw : tp->wd.layers) free_layer(lw);
-}
-
-static void free_train_state(w2l_ctx* ctx) {
-    TrainState* ts = ctx->train;
-    if (!ts) return;
-    for (auto& kv : ts->plans) free_train_plan(kv.second.get());
-    for (int n = 0; n < 3; ++n) {
-        for (float* p : ts->adam[n].m) cudaFree(p);
-        for (float* p : ts->adam[n].v) cudaFree(p);
-        if (ts->adam[n].dev) cudaFree(ts->adam[n].dev);
-    }
-    for (float* p : {ts->loss_dev, ts->a_emb, ts->v_emb, ts->da, ts->dv, ts->g_buf, ts->dg_buf, ts->prob, ts->dprob})
-        if (p) cudaFree(p);
-    if (ts->comm && ts->comm_destroy) ts->comm_destroy(ts->comm);
-    if (ts->s_comm) cudaStreamDestroy(ts->s_comm);
-    if (ts->ev_bucket) cudaEventDestroy(ts->ev_bucket);
-    if (ts->ev_comm) cudaEventDestroy(ts->ev_comm);
-    if (ts->s_wg) cudaStreamDestroy(ts->s_wg);
-    for (cudaEvent_t e : {ts->ev_dz, ts->ev_wg, ts->ev_wgb, ts->ev_aux_fork, ts->ev_aux_join, ts->ev_disc_fork, ts->ev_disc_join})
-        if (e) cudaEventDestroy(e);
-    if (ts->s_aux) cudaStreamDestroy(ts->s_aux);
-    if (ts->s_disc) cudaStreamDestroy(ts->s_disc);
-    delete ts;
-    ctx->train = nullptr;
+    if (!ctx->train) ctx->train.reset(new TrainState());
+    return ctx->train.get();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -198,18 +170,17 @@ static int load_dgrad_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const Laye
     }
     // stride 1: dst[tap][ci][co] = W[co][ci][r][s], tap (r,s) reads dz at (y + ph - r, x + pw - s)
     // (Ld.cout may have been widened to a multiple of 128 — see dgrad_layer — the extra rows are zero and never stored)
-    free_layer(*lw);
+    *lw = LayerW();
     std::vector<std::pair<int, int>> rs;
     PackedW pw;
     for (int r = 0; r < L.kh; ++r)
         for (int s = 0; s < L.kw; ++s) { rs.push_back({r, s}); pw.dy.push_back((signed char)(L.ph - r)); pw.dx.push_back((signed char)(L.pw - s)); }
-    CKR(pack_taps(ctx, &pw, W, L.cin, L.cout, L.kh, L.kw, true, rs, Ld.cout, log, st));
+    CKR(pack_taps(ctx, lw, &pw, W, L.cin, L.cout, L.kh, L.kw, true, rs, Ld.cout, log, st));
     lw->ph.push_back(pw);
     const int n_pad = Ld.cout;
-    void* sc = nullptr; void* sh = nullptr;
-    CKR(dev_alloc(&sc, (size_t)n_pad * 4));
-    CKR(dev_alloc(&sh, (size_t)n_pad * 4));
-    lw->scale = (float*)sc; lw->shift = (float*)sh; lw->n_scale = n_pad;
+    CKR(alloc_in(ctx, &lw->mem, &lw->scale, (size_t)n_pad * 4));
+    CKR(alloc_in(ctx, &lw->mem, &lw->shift, (size_t)n_pad * 4));
+    lw->n_scale = n_pad;
     fold_bn_kernel<<<(n_pad + 127) / 128, 128, 0, st>>>(nullptr, nullptr, nullptr, nullptr, nullptr, 1e-5f, n_pad, 1, n_pad, lw->scale, lw->shift);
     ctx->launches++;
     CK(cudaGetLastError());
@@ -391,10 +362,9 @@ static int add_train_block(w2l_ctx* ctx, TrainPlan* tp, int net, int li, const L
     // ---- statistics / reduction buffers ----
     const int rows = kBnThreads / (L.cout / 8);
     b.nblk = (int)std::max<long long>(1, std::min<long long>((b.M + rows - 1) / rows, (long long)ctx->num_sms * 4));
-    void* p = nullptr;
-    CKR(plan_alloc(&tp->pl, &p, (size_t)b.nblk * 2 * L.cout * 4)); b.partial = (float*)p;
-    CKR(plan_alloc(&tp->pl, &p, (size_t)4 * L.cout * 4)); b.stats = (float*)p;   // mean, invstd, G, H
-    CKR(plan_alloc(&tp->pl, &p, (size_t)3 * L.cout * 4)); b.coef = (float*)p;
+    CKR(plan_alloc(&tp->pl, &b.partial, (size_t)b.nblk * 2 * L.cout * 4));
+    CKR(plan_alloc(&tp->pl, &b.stats, (size_t)4 * L.cout * 4));   // mean, invstd, G, H
+    CKR(plan_alloc(&tp->pl, &b.coef, (size_t)3 * L.cout * 4));
     // ---- backward ----
     CKR(tp_act(tp, &b.dz, y.N, y.H, y.W, L.cout));
     if (b.bn && L.residual) CKR(tp_act(tp, &b.du, y.N, y.H, y.W, L.cout));
@@ -526,9 +496,7 @@ static int build_generator_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_ne
     CKR(tp_act(tp, &tp->dy32, N, 96, 96, 32));
     CKR(add_train_block(ctx, tp, net, g.output_block0, g.layers[g.output_block0], x, tp->y32, tp->dy32, dx, none, true, false, ws_need));
     tp->head_blocks = ctx->num_sms * 2;
-    void* p = nullptr;
-    CKR(plan_alloc(&tp->pl, &p, (size_t)tp->head_blocks * 99 * 4));
-    tp->head_partial = (float*)p;
+    CKR(plan_alloc(&tp->pl, &tp->head_partial, (size_t)tp->head_blocks * 99 * 4));
     return W2L_OK;
 }
 
@@ -542,9 +510,8 @@ static int build_syncnet_train_plan(w2l_ctx* ctx, TrainPlan* tp, size_t* ws_need
     syncnet_inputs(N, tp->T, &mel, &face);
     add_train_ingest(tp, "ingest.mel", mel, melIn);
     add_train_ingest(tp, tp->T > 0 ? "ingest.frames" : "ingest.face", face, faceIn);
-    void* p = nullptr;
-    CKR(plan_alloc(&tp->pl, &p, (size_t)N * 512 * 4)); tp->fe_raw = (float*)p;
-    CKR(plan_alloc(&tp->pl, &p, (size_t)N * 512 * 4)); tp->ae_raw = (float*)p;
+    CKR(plan_alloc(&tp->pl, &tp->fe_raw, (size_t)N * 512 * 4));
+    CKR(plan_alloc(&tp->pl, &tp->ae_raw, (size_t)N * 512 * 4));
     if (input_grad) CKR(tp_act(tp, &tp->dface_in, N, 48, 96, 16));
     Act ae, fe;
     CKR(add_train_chain(ctx, tp, net, s.layers, s.audio_enc, melIn, none, none, nullptr, nullptr, want_wgrad, ws_need, &ae, &tp->dae, tp->ae_raw));
@@ -581,7 +548,7 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
     snprintf(key, sizeof(key), "%d:%d:%d:%d:%d", net, B, T, (int)want_wgrad, (int)input_grad);
     auto it = ts->plans.find(key);
     if (it != ts->plans.end()) { *out = it->second.get(); return W2L_OK; }
-    std::unique_ptr<TrainPlan> tp(new TrainPlan());
+    std::unique_ptr<TrainPlan> tp(new TrainPlan(ctx));
     tp->net = net; tp->B = B; tp->T = T; tp->input_grad = input_grad;
     tp->N = (net == W2L_NET_SYNCNET) ? B : (T > 0 ? B * T : B);
     size_t ws_need[2] = {0, 0};
@@ -589,13 +556,12 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
     if (net == W2L_NET_GENERATOR) r = build_generator_train_plan(ctx, tp.get(), ws_need);
     else if (net == W2L_NET_SYNCNET) r = build_syncnet_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
     else r = build_disc_train_plan(ctx, tp.get(), ws_need, want_wgrad, input_grad);
-    for (int lane = 0; lane < 2 && r == W2L_OK; ++lane) {
+    CKR(r);
+    for (int lane = 0; lane < 2; ++lane) {
         if (!ws_need[lane]) continue;
-        void* p = nullptr;
-        r = plan_alloc(&tp->pl, &p, ws_need[lane]);
-        tp->wg_ws[lane] = (float*)p; tp->wg_ws_bytes[lane] = ws_need[lane];
+        CKR(plan_alloc(&tp->pl, &tp->wg_ws[lane], ws_need[lane]));
+        tp->wg_ws_bytes[lane] = ws_need[lane];
     }
-    if (r != W2L_OK) { free_train_plan(tp.get()); return r; }
     CK(cudaDeviceSynchronize());
     *out = tp.get();
     ts->plans[key] = std::move(tp);
@@ -608,7 +574,7 @@ static int get_train_plan(w2l_ctx* ctx, int net, int B, int T, bool want_wgrad, 
 static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
     const std::vector<PackParams>& jobs = tp->repack.pack;
     if (!jobs.empty()) {
-        if (!tp->pack_dev) {   // job table + block map, built once per plan
+        if (!tp->pack_blocks) {   // job table + block map, built once per plan
             std::vector<int> blk_job, blk_first;
             for (size_t j = 0; j < jobs.size(); ++j) {
                 const PackParams& pp = jobs[j];
@@ -616,10 +582,9 @@ static int repack_weights(w2l_ctx* ctx, TrainPlan* tp, cudaStream_t st) {
                 blk_first.push_back((int)blk_job.size());
                 for (long long b = 0; b < (total + 4095) / 4096; ++b) blk_job.push_back((int)j);
             }
-            void* d = nullptr;
-            CKR(plan_alloc(&tp->pl, &d, jobs.size() * sizeof(PackParams))); tp->pack_dev = (PackParams*)d;
-            CKR(plan_alloc(&tp->pl, &d, blk_job.size() * 4)); tp->pack_blk_job = (int*)d;
-            CKR(plan_alloc(&tp->pl, &d, blk_first.size() * 4)); tp->pack_blk_first = (int*)d;
+            CKR(tp->pack_dev.grow(ctx, jobs.size() * sizeof(PackParams)));
+            CKR(tp->pack_blk_job.grow(ctx, blk_job.size() * 4));
+            CKR(tp->pack_blk_first.grow(ctx, blk_first.size() * 4));
             CK(cudaMemcpy(tp->pack_dev, jobs.data(), jobs.size() * sizeof(PackParams), cudaMemcpyHostToDevice));
             CK(cudaMemcpy(tp->pack_blk_job, blk_job.data(), blk_job.size() * 4, cudaMemcpyHostToDevice));
             CK(cudaMemcpy(tp->pack_blk_first, blk_first.data(), blk_first.size() * 4, cudaMemcpyHostToDevice));
@@ -678,25 +643,25 @@ static int block_forward(w2l_ctx* ctx, TrainPlan* tp, TBlock& b, bool update_run
 
 static int ensure_wg_stream(TrainState* ts) {
     if (ts->s_wg) return W2L_OK;
-    CK(cudaStreamCreateWithFlags(&ts->s_wg, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ts->ev_dz, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&ts->ev_wg, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&ts->ev_wgb, cudaEventDisableTiming));
+    CKR(ts->s_wg.create());
+    CKR(ts->ev_dz.create());
+    CKR(ts->ev_wg.create());
+    CKR(ts->ev_wgb.create());
     return W2L_OK;
 }
 
 static int ensure_aux_stream(TrainState* ts) {
     if (ts->s_aux) return W2L_OK;
-    CK(cudaStreamCreateWithFlags(&ts->s_aux, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ts->ev_aux_fork, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&ts->ev_aux_join, cudaEventDisableTiming));
+    CKR(ts->s_aux.create());
+    CKR(ts->ev_aux_fork.create());
+    CKR(ts->ev_aux_join.create());
     return W2L_OK;
 }
 static int ensure_disc_stream(TrainState* ts) {
     if (ts->s_disc) return W2L_OK;
-    CK(cudaStreamCreateWithFlags(&ts->s_disc, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ts->ev_disc_fork, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&ts->ev_disc_join, cudaEventDisableTiming));
+    CKR(ts->s_disc.create());
+    CKR(ts->ev_disc_fork.create());
+    CKR(ts->ev_disc_join.create());
     return W2L_OK;
 }
 static bool has_aux_lane(const TrainPlan* tp) {
@@ -900,28 +865,12 @@ static int train_backward(w2l_ctx* ctx, TrainPlan* tp, const float* d0, const fl
 // ------------------------------------------------------------------------------------------------
 static int ensure_train_scratch(w2l_ctx* ctx, int B, int T) {
     TrainState* ts = train_state(ctx);
-    void* p = nullptr;
-    if (!ts->loss_dev) { CKR(dev_alloc(&p, 2048 * 4)); ts->loss_dev = (float*)p; CK(cudaMemset(p, 0, 2048 * 4)); }
+    if (!ts->loss_dev) { CKR(ts->loss_dev.grow(ctx, 2048 * 4)); CK(cudaMemset(ts->loss_dev, 0, 2048 * 4)); }
     const int N = B * std::max(T, 1);
-    if (ts->emb_cap < B) {
-        CK(cudaDeviceSynchronize());
-        for (float** q : {&ts->a_emb, &ts->v_emb, &ts->da, &ts->dv}) { if (*q) cudaFree(*q); CKR(dev_alloc(&p, (size_t)B * 512 * 4)); *q = (float*)p; }
-        ts->emb_cap = B;
-    }
-    if (ts->prob_cap < N) {
-        CK(cudaDeviceSynchronize());
-        if (ts->prob) cudaFree(ts->prob);
-        if (ts->dprob) cudaFree(ts->dprob);
-        CKR(dev_alloc(&p, (size_t)2 * N * 4)); ts->prob = (float*)p;
-        CKR(dev_alloc(&p, (size_t)3 * N * 4)); ts->dprob = (float*)p;
-        ts->prob_cap = N;
-    }
-    const size_t gn = (size_t)N * 3 * 9216;
-    if (ts->g_cap < gn) {
-        CK(cudaDeviceSynchronize());
-        for (float** q : {&ts->g_buf, &ts->dg_buf}) { if (*q) cudaFree(*q); CKR(dev_alloc(&p, gn * 4)); *q = (float*)p; }
-        ts->g_cap = gn;
-    }
+    for (DevMem<float>* q : {&ts->a_emb, &ts->v_emb, &ts->da, &ts->dv}) CKR(q->grow(ctx, (size_t)B * 512 * 4));
+    CKR(ts->prob.grow(ctx, (size_t)2 * N * 4));
+    CKR(ts->dprob.grow(ctx, (size_t)3 * N * 4));
+    for (DevMem<float>* q : {&ts->g_buf, &ts->dg_buf}) CKR(q->grow(ctx, (size_t)N * 3 * 9216 * 4));
     return W2L_OK;
 }
 
@@ -930,23 +879,23 @@ static int ensure_adam_slot(w2l_ctx* ctx, int net, cudaStream_t st) {
     TrainState* ts = train_state(ctx);
     AdamSlot& a = ts->adam[net];
     if (a.dev) return W2L_OK;
+    AdamSlot t;   // stored in the slot only once every allocation has succeeded
     for (auto& kv : ts->bound[net]) {
         if (!kv.second.grad) continue;
-        void *m = nullptr, *v = nullptr;
-        CKR(dev_alloc(&m, (size_t)kv.second.n * 4));
-        CKR(dev_alloc(&v, (size_t)kv.second.n * 4));
-        CK(cudaMemsetAsync(m, 0, (size_t)kv.second.n * 4, st));
-        CK(cudaMemsetAsync(v, 0, (size_t)kv.second.n * 4, st));
-        a.names.push_back(kv.first);
-        a.m.push_back((float*)m); a.v.push_back((float*)v);
-        a.host.push_back(AdamTensor{kv.second.value, kv.second.grad, (float*)m, (float*)v, kv.second.n});
+        const size_t bytes = (size_t)kv.second.n * 4;
+        float *m, *v;
+        CKR(alloc_in(ctx, &t.moments, &m, bytes));
+        CKR(alloc_in(ctx, &t.moments, &v, bytes));
+        CK(cudaMemsetAsync(m, 0, bytes, st));
+        CK(cudaMemsetAsync(v, 0, bytes, st));
+        t.names.push_back(kv.first);
+        t.host.push_back(AdamTensor{kv.second.value, kv.second.grad, m, v, kv.second.n});
     }
-    if (a.host.empty()) return fail(W2L_ESTATE, "adam: no gradient tensors bound for net %d", net);
-    void* d = nullptr;
-    CKR(dev_alloc(&d, a.host.size() * sizeof(AdamTensor)));
-    a.dev = (AdamTensor*)d;
-    CK(cudaMemcpyAsync(a.dev, a.host.data(), a.host.size() * sizeof(AdamTensor), cudaMemcpyHostToDevice, st));
+    if (t.host.empty()) return fail(W2L_ESTATE, "adam: no gradient tensors bound for net %d", net);
+    CKR(t.dev.grow(ctx, t.host.size() * sizeof(AdamTensor)));
+    CK(cudaMemcpyAsync(t.dev, t.host.data(), t.host.size() * sizeof(AdamTensor), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
+    a = std::move(t);
     return W2L_OK;
 }
 

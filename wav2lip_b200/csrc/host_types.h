@@ -1,5 +1,6 @@
 // host_types.h — host-side data model of libw2l.so: error reporting, the architecture specs, the tensor-map encoder entry
-// point, activation views (Act), packed weights, launch descriptors (Op), plans and the context.
+// point, owning handles (device memory, streams, events), activation views (Act), packed weights, launch descriptors (Op),
+// plans and the context.
 // Part of the single translation unit w2l_api.cu (included there, in this order).
 #pragma once
 
@@ -66,6 +67,64 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 // ------------------------------------------------------------------------------------------------
+// owning handles
+// ------------------------------------------------------------------------------------------------
+// Every device buffer, stream and event belongs to one of these, held by the context, a plan, a weight layer or the
+// training state, and is released when its holder is destroyed.  Releases run with the context's device current: every
+// entry point holds a DeviceGuard.
+struct DeviceGuard {
+    int prev = -1;
+    explicit DeviceGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
+    ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+static int dev_alloc(void** p, size_t bytes) {
+    cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) return W2L_OK;
+    cudaGetLastError();  // a failed allocation is not sticky: clear it, or the next launch check reports it again
+    *p = nullptr;
+    return fail(W2L_ENOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+}
+
+struct w2l_ctx;
+
+// One cudaMalloc block, counted on its context's device_bytes while it is held.
+template <class T = void>
+struct DevMem {
+    T* p = nullptr;
+    size_t cap = 0;              // bytes
+    size_t* counter = nullptr;   // &w2l_ctx::device_bytes
+    DevMem() = default;
+    DevMem(DevMem&& o) noexcept : p(o.p), cap(o.cap), counter(o.counter) { o.p = nullptr; o.cap = 0; }
+    DevMem& operator=(DevMem&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); std::swap(counter, o.counter); return *this; }
+    ~DevMem() { if (p) { cudaFree(p); *counter -= cap; } }
+    operator T*() const { return p; }
+    // at least `bytes`: a smaller block is released once the device is idle (queued work may still read it) and
+    // replaced; when that allocation fails the block is left empty
+    int grow(w2l_ctx* ctx, size_t bytes);
+};
+
+struct Stream {
+    cudaStream_t h = nullptr;
+    Stream() = default;
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() { if (h) cudaStreamDestroy(h); }
+    int create() { CK(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking)); return W2L_OK; }
+    operator cudaStream_t() const { return h; }
+};
+
+struct Event {
+    cudaEvent_t h = nullptr;
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { if (h) cudaEventDestroy(h); }
+    int create(unsigned flags = cudaEventDisableTiming) { CK(cudaEventCreateWithFlags(&h, flags)); return W2L_OK; }
+    operator cudaEvent_t() const { return h; }
+};
+
+// ------------------------------------------------------------------------------------------------
 // tensors in HBM
 // ------------------------------------------------------------------------------------------------
 // Activations are NHWC, 16-bit (fp16 or bf16), channel pitch Cs; a view may select a channel slice
@@ -102,6 +161,7 @@ struct LayerW {
     std::vector<PackedW> ph;  // 1 for conv, 4 for stride-2 convT, 1 (as GEMM) for the 1x1->3x3 convT
     float* scale = nullptr;
     float* shift = nullptr;
+    std::vector<DevMem<>> mem;  // the slabs of ph, scale and shift
     int n_scale = 0;
     bool gemm_convT = false;
     bool has_all_taps = false;  // ph.back() holds all 9 taps of a stride-2 transposed conv (fused 4-phase kernel)
@@ -110,8 +170,8 @@ struct LayerW {
 
 struct NetW {
     std::vector<LayerW> layers;
-    float* head_w = nullptr;  // generator output_block.1 (3x32) / disc binary_pred (512)
-    float* head_b = nullptr;
+    DevMem<float> head_w;  // generator output_block.1 (3x32) / disc binary_pred (512)
+    DevMem<float> head_b;
     bool loaded = false;
 };
 
@@ -155,11 +215,12 @@ struct S3fdDetWork {
 };
 
 struct Plan {
+    explicit Plan(w2l_ctx* c) : ctx(c) {}
+    w2l_ctx* ctx;                  // its allocations count on this context's device_bytes
     int net = 0, B = 0, T = 0, N = 0;
     int H = 0, W = 0;              // S3FD: image size
     std::vector<Op> ops;
-    std::vector<void*> allocs;
-    size_t bytes = 0;
+    std::vector<DevMem<>> allocs;
     std::map<int, Act> layer_out;  // layer index -> activation view (debug export)
     long long last_used = 0;       // LRU stamp
     bool x2 = false;               // split-operand precision: activations carry hi and lo planes
@@ -174,7 +235,7 @@ struct RepackLog { std::vector<PackParams> pack; std::vector<PackFoldParams> pac
 struct TrainState;  // host_train.cuh
 
 struct w2l_ctx {
-    TrainState* train = nullptr;
+    size_t device_bytes = 0;   // every block the members below hold (w2l_device_bytes); declared first, destroyed last
     int device = 0;
     bool bf16 = false;
     bool x2 = false;        // W2L_PREC_F32X: split fp16 operands (hi + lo), generic kernel only
@@ -190,56 +251,66 @@ struct w2l_ctx {
     bool use_fold = true;   // W2L_DISABLE_FOLD=1 / driver rejects overlapping-stride tensor maps
     bool use_pdl = true;      // W2L_DISABLE_PDL=1
     NetW nets[4];
-    float* s3fd_l2w[3] = {nullptr, nullptr, nullptr};   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)
+    DevMem<float> s3fd_l2w[3];   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)
     std::map<std::string, std::unique_ptr<Plan>> plans;
     Plan* last_plan[4] = {nullptr, nullptr, nullptr, nullptr};
     std::vector<w2l_kernel_info> last_block_kernels;  // conv launches of the last w2l_conv_block_forward (its plan is freed)
     int64_t launches = 0;
     long long plan_clock = 0;
-    size_t weight_bytes = 0;
     // host-buffer entry points: compute stream + copy streams, double-buffered device staging
-    cudaStream_t stream = nullptr;
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
-    cudaStream_t s_side = nullptr;   // audio-encoder lane of the generator plan
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    Stream stream;
+    Stream s_h2d, s_d2h;
+    Stream s_side;                   // audio-encoder lane of the generator plan
+    Event ev_fork, ev_join;
     bool use_side = true;            // W2L_DISABLE_SIDESTREAM=1
-    cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-    void* stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    int* boxes_dev = nullptr; int box_cap = 0;                 // crop / paste boxes (row f2)
-    int* samples_dev = nullptr; size_t sample_cap = 0;         // training-batch sample table (ints)
-    uint8_t *crops_dev = nullptr, *preds_dev = nullptr; size_t crop_cap = 0;
-    float* scratch = nullptr;  // partial sums of the loss kernels
-    size_t scratch_bytes = 0;
+    Event ev_in[2], ev_done[2], ev_out[2];
+    DevMem<> stage[6];
+    DevMem<int> boxes_dev;           // crop / paste boxes (row f2)
+    DevMem<int> samples_dev;         // training-batch sample table (ints)
+    DevMem<uint8_t> crops_dev, preds_dev;
+    DevMem<float> scratch;           // partial sums of the loss kernels
     long long host_seq = 0;   // host-buffer submissions so far (staging slot = seq & 1)
     int host_inflight = 0;    // submitted and not yet retired by host_drain
-    size_t stage_bytes[6] = {0, 0, 0, 0, 0, 0};
     // mel tables
-    double2* mel_tw = nullptr;
-    float* mel_bvals = nullptr;
-    int* mel_boff = nullptr;
-    int* mel_bstart = nullptr;
-    int* mel_blen = nullptr;
+    DevMem<double2> mel_tw;
+    DevMem<float> mel_bvals;
+    DevMem<int> mel_boff;
+    DevMem<int> mel_bstart;
+    DevMem<int> mel_blen;
+    std::unique_ptr<TrainState> train;   // declared last: released first
 };
 
-static int dev_alloc(void** p, size_t bytes) {
-    cudaError_t e = cudaMalloc(p, bytes ? bytes : 16);
-    if (e != cudaSuccess) return fail(W2L_ENOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+template <class T>
+int DevMem<T>::grow(w2l_ctx* ctx, size_t bytes) {
+    if (p && cap >= bytes) return W2L_OK;
+    if (p) {
+        CK(cudaDeviceSynchronize());
+        *this = DevMem();
+    }
+    const size_t n = bytes ? bytes : 16;
+    void* q;
+    CKR(dev_alloc(&q, n));
+    p = (T*)q; cap = n; counter = &ctx->device_bytes;
+    *counter += n;
     return W2L_OK;
 }
 
-static int plan_alloc(Plan* pl, void** p, size_t bytes) {
-    CKR(dev_alloc(p, bytes));
-    pl->allocs.push_back(*p);
-    pl->bytes += bytes;
+// a new block of `bytes`, held by `owner`
+template <class T>
+static int alloc_in(w2l_ctx* ctx, std::vector<DevMem<>>* owner, T** p, size_t bytes) {
+    owner->emplace_back();
+    CKR(owner->back().grow(ctx, bytes));
+    *p = (T*)owner->back().p;
     return W2L_OK;
 }
+
+template <class T>
+static int plan_alloc(Plan* pl, T** p, size_t bytes) { return alloc_in(pl->ctx, &pl->allocs, p, bytes); }
 
 static int plan_act(Plan* pl, Act* a, int N, int H, int W, int C, bool f32 = false) {
-    void* p = nullptr;
     const bool planes = pl->x2 && !f32;
     const size_t bytes = (size_t)N * H * W * C * (f32 ? 4 : 2) * (planes ? 2 : 1);
-    CKR(plan_alloc(pl, &p, bytes));
-    a->base = (uint16_t*)p;
+    CKR(plan_alloc(pl, &a->base, bytes));
     a->N = N; a->H = H; a->W = W; a->Cs = planes ? 2 * C : C; a->c_off = 0; a->C = C; a->f32 = f32;
     a->lo_off = planes ? C : 0;
     return W2L_OK;
@@ -253,18 +324,11 @@ static int plan_input_act(Plan* pl, Act* a, int N, int H, int W, int cin, const 
     if (!w.fold) return plan_act(pl, a, N, H, W, ((cin + 15) / 16) * 16);
     const int Wout = (W + 2 * L.pw - L.kw) / L.sw + 1;
     const int Wp = (std::max(W + L.pw, (Wout - 1) * L.sw + w.win) + 1) / 2 * 2;
-    void* p = nullptr;
     const size_t bytes = ((size_t)N * H * Wp * w.Cp + w.kfold) * 2;  // + one window of slack at the very end
-    CKR(plan_alloc(pl, &p, bytes));
-    CK(cudaMemset(p, 0, bytes));
-    a->base = (uint16_t*)p;
+    CKR(plan_alloc(pl, &a->base, bytes));
+    CK(cudaMemset(a->base, 0, bytes));
     a->N = N; a->H = H; a->W = W; a->Cs = w.Cp; a->c_off = 0; a->C = w.kfold; a->f32 = false;
     a->Wp = Wp; a->x_off = L.pw;
     a->wstride = L.sw; a->nwin = Wout;
     return W2L_OK;
-}
-
-static void free_plan(Plan* pl) {
-    for (void* p : pl->allocs) cudaFree(p);
-    pl->allocs.clear();
 }

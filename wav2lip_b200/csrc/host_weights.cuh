@@ -17,8 +17,9 @@ static int need(const TensorMap& tm, const std::string& name, int64_t numel, con
     return W2L_OK;
 }
 
-// log != nullptr (training): the job is also recorded there, to be replayed after every optimizer step
-static int pack_taps(w2l_ctx* ctx, PackedW* pw, const float* src, int cout, int cin, int kh, int kw, bool transposed,
+// The slabs go to lw's memory.  log != nullptr (training): the job is also recorded there, to be replayed after every
+// optimizer step
+static int pack_taps(w2l_ctx* ctx, LayerW* lw, PackedW* pw, const float* src, int cout, int cin, int kh, int kw, bool transposed,
                      const std::vector<std::pair<int, int>>& rs, int cout_pad_to, RepackLog* log, cudaStream_t st,
                      uint16_t* dst_override = nullptr) {
     PackParams pp;
@@ -36,10 +37,7 @@ static int pack_taps(w2l_ctx* ctx, PackedW* pw, const float* src, int cout, int 
     const int planes = (ctx->x2 && !dst_override) ? 2 : 1;
     if (dst_override) pp.dst = dst_override;
     else {
-        void* d = nullptr;
-        CKR(dev_alloc(&d, n * 2 * planes));
-        ctx->weight_bytes += n * 2 * planes;
-        pp.dst = (uint16_t*)d;
+        CKR(alloc_in(ctx, &lw->mem, &pp.dst, n * 2 * planes));
         pw->w = pp.dst;
         pw->ntaps = pp.ntaps; pw->cout_pad = pp.cout_pad; pw->cin_pad = pp.cin_pad;
         pw->nslabs = pp.ntaps * planes;
@@ -57,23 +55,12 @@ static int pack_taps(w2l_ctx* ctx, PackedW* pw, const float* src, int cout, int 
     return W2L_OK;
 }
 
-static void free_layer(LayerW& lw) {
-    for (auto& p : lw.ph) if (p.w) cudaFree(p.w);
-    lw.ph.clear();
-    if (lw.scale) cudaFree(lw.scale);
-    if (lw.shift) cudaFree(lw.shift);
-    lw.scale = lw.shift = nullptr;
-    lw.loaded = false;
-    lw.has_all_taps = false;
-    lw.gemm_convT = false;
-}
-
 // Pack one block's parameters. in_hw1: the block is applied to a 1x1 input (enables the GEMM form of convT).
 //   fold: the block may read a K-folded input (first layers fed by the ingest kernel);  log: see pack_taps
 static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, const float* bias, const float* gamma,
                       const float* beta, const float* mean, const float* var, bool in_hw1, bool fold, RepackLog* log,
                       cudaStream_t st) {
-    free_layer(*lw);
+    *lw = LayerW();
     const int pad_to = 16;
     int reps = 1;
     if (fold && L.kind != W2L_BLOCK_CONVT_BN_RELU && L.cin <= 16 && L.kw >= 3 && (L.sw == 1 || L.sw == 2)) {
@@ -87,10 +74,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         pw.ntaps = L.kh; pw.cin_pad = pw.kfold; pw.cout_pad = round_up(L.cout, pad_to);
         for (int r = 0; r < L.kh; ++r) { pw.dy.push_back((signed char)(r - L.ph)); pw.dx.push_back(0); }
         const size_t n = (size_t)pw.ntaps * pw.cout_pad * pw.kfold;
-        void* d = nullptr;
-        CKR(dev_alloc(&d, n * 2));
-        ctx->weight_bytes += n * 2;
-        pw.w = (uint16_t*)d;
+        CKR(alloc_in(ctx, &lw->mem, &pw.w, n * 2));
         PackFoldParams fp;
         fp.src = W; fp.dst = pw.w; fp.kh = L.kh; fp.kw = L.kw; fp.cout = L.cout; fp.cin = L.cin;
         fp.cout_pad = pw.cout_pad; fp.kfold = pw.kfold; fp.Cp = pw.Cp;
@@ -106,7 +90,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         PackedW pw;
         for (int r = 0; r < L.kh; ++r)
             for (int s = 0; s < L.kw; ++s) { rs.push_back({r, s}); pw.dy.push_back((signed char)(r - L.ph)); pw.dx.push_back((signed char)(s - L.pw)); }
-        CKR(pack_taps(ctx, &pw, W, L.cout_real > 0 ? L.cout_real : L.cout, L.cin, L.kh, L.kw, false, rs, pad_to, log, st));
+        CKR(pack_taps(ctx, lw, &pw, W, L.cout_real > 0 ? L.cout_real : L.cout, L.cin, L.kh, L.kw, false, rs, pad_to, log, st));
         lw->ph.push_back(pw);
     } else if (in_hw1 && !ctx->x2 && L.sh == 1 && L.sw == 1 && L.ph == 0 && L.pw == 0) {
         // out[n, y, x, co] = sum_ci in[n, ci] * W[ci, co, y, x]  -> GEMM with columns (y, x, co)
@@ -115,16 +99,12 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
         PackedW pw;
         pw.ntaps = 1; pw.cin_pad = round_up(L.cin, 16); pw.cout_pad = round_up(L.cout, pad_to) * reps;
         pw.dx.push_back(0); pw.dy.push_back(0);
-        void* d = nullptr;
-        const size_t n = (size_t)pw.cout_pad * pw.cin_pad;
-        CKR(dev_alloc(&d, n * 2));
-        ctx->weight_bytes += n * 2;
-        pw.w = (uint16_t*)d;
+        CKR(alloc_in(ctx, &lw->mem, &pw.w, (size_t)pw.cout_pad * pw.cin_pad * 2));
         if (L.cout % pad_to != 0) return fail(W2L_EINVAL, "%s: gemm convT needs cout %% 16 == 0", L.name.c_str());
         for (int r = 0; r < L.kh; ++r)
             for (int s = 0; s < L.kw; ++s) {
                 std::vector<std::pair<int, int>> rs = {{r, s}};
-                CKR(pack_taps(ctx, nullptr, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st,
+                CKR(pack_taps(ctx, lw, nullptr, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st,
                               pw.w + (size_t)(r * L.kw + s) * L.cout * pw.cin_pad));
             }
         lw->ph.push_back(pw);
@@ -145,7 +125,7 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
                     }
                 }
                 if (rs.empty()) return fail(W2L_EINVAL, "%s: empty transposed-conv phase", L.name.c_str());
-                CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
+                CKR(pack_taps(ctx, lw, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
                 lw->ph.push_back(pw);
             }
         if (!ctx->x2 && L.cout == kCtBN && L.kh == 3 && L.kw == 3 && L.sh == 2 && L.sw == 2 && L.ph == 1 && L.pw == 1 && L.out_pad == 1) {
@@ -158,16 +138,15 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
                                                    {0, 0}};                          // shift (1,1): phase 11
             PackedW pw;
             for (int t = 0; t < 9; ++t) { pw.dy.push_back(0); pw.dx.push_back(0); }
-            CKR(pack_taps(ctx, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
+            CKR(pack_taps(ctx, lw, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
             lw->ph.push_back(pw);
             lw->has_all_taps = true;
         }
     }
     const int n_pad = round_up(L.cout, pad_to) * reps;
-    void* sc = nullptr; void* sh = nullptr;
-    CKR(dev_alloc(&sc, (size_t)n_pad * 4));
-    CKR(dev_alloc(&sh, (size_t)n_pad * 4));
-    lw->scale = (float*)sc; lw->shift = (float*)sh; lw->n_scale = n_pad;
+    CKR(alloc_in(ctx, &lw->mem, &lw->scale, (size_t)n_pad * 4));
+    CKR(alloc_in(ctx, &lw->mem, &lw->shift, (size_t)n_pad * 4));
+    lw->n_scale = n_pad;
     fold_bn_kernel<<<(n_pad + 127) / 128, 128, 0, st>>>(bias, gamma, beta, mean, var, 1e-5f, L.cout_real > 0 ? L.cout_real : L.cout, reps, n_pad, lw->scale, lw->shift);
     if (log && bias) log->fold.push_back(FoldJob{bias, L.cout, reps, n_pad, lw->scale, lw->shift});
     ctx->launches++;
@@ -194,7 +173,7 @@ static int fetch_block_tensors(const TensorMap& tm, const Layer& L, const float*
 
 static void drop_plans(w2l_ctx* ctx, int net) {
     for (auto it = ctx->plans.begin(); it != ctx->plans.end();) {
-        if (it->second->net == net) { free_plan(it->second.get()); it = ctx->plans.erase(it); }
+        if (it->second->net == net) it = ctx->plans.erase(it);
         else ++it;
     }
     ctx->last_plan[net] = nullptr;

@@ -88,25 +88,16 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
     if (prop.major != 9 || prop.minor != 0) return fail(W2L_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     if (!get_encode_fn()) return fail(W2L_ENODEV, "cuTensorMapEncodeTiled not found in the driver");
     DeviceGuard g(device);
-    w2l_ctx* ctx = new w2l_ctx();
+    std::unique_ptr<w2l_ctx> ctx(new w2l_ctx());   // released here, device current, if anything below fails
     ctx->device = device;
     ctx->bf16 = precision == W2L_PREC_BF16;
     ctx->x2 = precision == W2L_PREC_F32X;
     ctx->num_sms = prop.multiProcessorCount;
-    cudaError_t e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->s_side, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming);
-    for (int i = 0; i < 2 && e == cudaSuccess; ++i) {
-        e = cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_out[i], cudaEventDisableTiming);
-    }
-    if (e != cudaSuccess) { w2l_destroy(ctx); return fail(W2L_ECUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
-    int r = init_mel_tables(ctx);
-    if (r != W2L_OK) { const std::string msg = g_err; w2l_destroy(ctx); g_err = msg; return r; }
+    for (Stream* s : {&ctx->stream, &ctx->s_h2d, &ctx->s_d2h, &ctx->s_side}) CKR(s->create());
+    for (Event* e : {&ctx->ev_fork, &ctx->ev_join, &ctx->ev_in[0], &ctx->ev_done[0], &ctx->ev_out[0], &ctx->ev_in[1],
+                     &ctx->ev_done[1], &ctx->ev_out[1]})
+        CKR(e->create());
+    CKR(init_mel_tables(ctx.get()));
     {
         // A/B switches, read once per context: W2L_DISABLE_<NAME>=1 turns one specialised path off (tests/test_gpu_variants.py)
         auto enabled = [](const char* name) { const char* v = getenv(name); return !(v && v[0] == '1'); };
@@ -127,12 +118,12 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
             // the folded first layers need a tensor map whose pixel stride (16 B) is smaller than its inner extent
             // (128 B): probe once that the driver encodes such overlapping windows
             Act probe;
-            probe.base = (uint16_t*)ctx->mel_tw; probe.N = 2; probe.H = 16; probe.W = 16; probe.Cs = 8; probe.C = 64; probe.Wp = 24;
+            probe.base = (uint16_t*)ctx->mel_tw.p; probe.N = 2; probe.H = 16; probe.W = 16; probe.Cs = 8; probe.C = 64; probe.Wp = 24;
             CUtensorMap tm;
-            if (encode_act_map(ctx, &tm, probe, 64, 8, 8, 2, 1, 1, "probe") != W2L_OK) { ctx->use_fold = false; g_err.clear(); }
+            if (encode_act_map(ctx.get(), &tm, probe, 64, 8, 8, 2, 1, 1, "probe") != W2L_OK) { ctx->use_fold = false; g_err.clear(); }
         }
     }
-    *out = ctx;
+    *out = ctx.release();
     return W2L_OK;
 }
 
@@ -140,32 +131,6 @@ int w2l_destroy(w2l_ctx* ctx) {
     if (!ctx) return W2L_OK;
     DeviceGuard g(ctx->device);
     cudaDeviceSynchronize();
-    free_train_state(ctx);
-    for (auto& kv : ctx->plans) free_plan(kv.second.get());
-    for (int i = 0; i < 3; ++i) if (ctx->s3fd_l2w[i]) cudaFree(ctx->s3fd_l2w[i]);
-    for (int n = 0; n < 4; ++n) {
-        for (auto& lw : ctx->nets[n].layers) free_layer(lw);
-        if (ctx->nets[n].head_w) cudaFree(ctx->nets[n].head_w);
-        if (ctx->nets[n].head_b) cudaFree(ctx->nets[n].head_b);
-    }
-    for (int i = 0; i < 6; ++i) if (ctx->stage[i]) cudaFree(ctx->stage[i]);
-    if (ctx->s_h2d) cudaStreamDestroy(ctx->s_h2d);
-    if (ctx->s_d2h) cudaStreamDestroy(ctx->s_d2h);
-    if (ctx->s_side) cudaStreamDestroy(ctx->s_side);
-    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-    for (int i = 0; i < 2; ++i) { if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]); if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]); if (ctx->ev_out[i]) cudaEventDestroy(ctx->ev_out[i]); }
-    if (ctx->scratch) cudaFree(ctx->scratch);
-    if (ctx->boxes_dev) cudaFree(ctx->boxes_dev);
-    if (ctx->samples_dev) cudaFree(ctx->samples_dev);
-    if (ctx->crops_dev) cudaFree(ctx->crops_dev);
-    if (ctx->preds_dev) cudaFree(ctx->preds_dev);
-    if (ctx->mel_tw) cudaFree(ctx->mel_tw);
-    if (ctx->mel_bvals) cudaFree(ctx->mel_bvals);
-    if (ctx->mel_boff) cudaFree(ctx->mel_boff);
-    if (ctx->mel_bstart) cudaFree(ctx->mel_bstart);
-    if (ctx->mel_blen) cudaFree(ctx->mel_blen);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return W2L_OK;
 }
@@ -208,8 +173,6 @@ int w2l_load_weights(w2l_ctx* ctx, int net, int n_tensors, const char* const* na
         if (net == W2L_NET_GENERATOR && L.name == "face_encoder_blocks.1.0" && ctx->use_patch && ctx->use_fold && ctx->use_fold_s2) first = true;
         CKR(load_layer(ctx, &nw.layers[i], L, W, b, gm, be, m, v, hw1, first && ctx->use_fold, nullptr, st));
     }
-    if (nw.head_w) { cudaFree(nw.head_w); nw.head_w = nullptr; }
-    if (nw.head_b) { cudaFree(nw.head_b); nw.head_b = nullptr; }
     if (net == W2L_NET_GENERATOR || net == W2L_NET_DISC) {
         const char* wn = net == W2L_NET_GENERATOR ? "output_block.1.weight" : "binary_pred.0.weight";
         const char* bn = net == W2L_NET_GENERATOR ? "output_block.1.bias" : "binary_pred.0.bias";
@@ -217,9 +180,8 @@ int w2l_load_weights(w2l_ctx* ctx, int net, int n_tensors, const char* const* na
         const float *hw, *hb;
         CKR(need(tm, wn, wcount, &hw));
         CKR(need(tm, bn, bcount, &hb));
-        void* p;
-        CKR(dev_alloc(&p, wcount * 4)); nw.head_w = (float*)p;
-        CKR(dev_alloc(&p, bcount * 4)); nw.head_b = (float*)p;
+        CKR(nw.head_w.grow(ctx, wcount * 4));
+        CKR(nw.head_b.grow(ctx, bcount * 4));
         CK(cudaMemcpyAsync(nw.head_w, hw, wcount * 4, cudaMemcpyDeviceToDevice, st));
         CK(cudaMemcpyAsync(nw.head_b, hb, bcount * 4, cudaMemcpyDeviceToDevice, st));
     }
@@ -229,7 +191,7 @@ int w2l_load_weights(w2l_ctx* ctx, int net, int n_tensors, const char* const* na
         for (int i = 0; i < 3; ++i) {
             const float* w;
             CKR(need(tm, names3[i], n3[i], &w));
-            if (!ctx->s3fd_l2w[i]) { void* p; CKR(dev_alloc(&p, 512 * 4)); ctx->s3fd_l2w[i] = (float*)p; }
+            CKR(ctx->s3fd_l2w[i].grow(ctx, 512 * 4));
             CK(cudaMemcpyAsync(ctx->s3fd_l2w[i], w, n3[i] * 4, cudaMemcpyDeviceToDevice, st));
         }
     }
@@ -264,11 +226,11 @@ static int host_submit(w2l_ctx* ctx, int B, int T, const void* mel_h, size_t mel
                        void* out_h, size_t out_bytes, bool u8) {
     if (ctx->host_inflight >= 2) CKR(host_drain(ctx, 1));
     const int sl = (int)(ctx->host_seq & 1);
-    if (ctx->stage_bytes[0 + sl] < mel_bytes || ctx->stage_bytes[2 + sl] < face_bytes || ctx->stage_bytes[4 + sl] < out_bytes) {
+    if (ctx->stage[0 + sl].cap < mel_bytes || ctx->stage[2 + sl].cap < face_bytes || ctx->stage[4 + sl].cap < out_bytes) {
         CKR(host_drain(ctx, 0));  // growing a staging buffer frees the old one
-        CKR(ensure_stage(ctx, 0 + sl, mel_bytes));
-        CKR(ensure_stage(ctx, 2 + sl, face_bytes));
-        CKR(ensure_stage(ctx, 4 + sl, out_bytes));
+        CKR(ctx->stage[0 + sl].grow(ctx, mel_bytes));
+        CKR(ctx->stage[2 + sl].grow(ctx, face_bytes));
+        CKR(ctx->stage[4 + sl].grow(ctx, out_bytes));
     }
     Plan* pl;
     CKR(get_plan(ctx, W2L_NET_GENERATOR, B, T, &pl));
@@ -362,13 +324,7 @@ static int upload_boxes(w2l_ctx* ctx, const int32_t* boxes, int N, int F, int H,
         if (b[0] < 0 || b[0] >= F || b[1] < 0 || b[2] > H || b[1] >= b[2] || b[3] < 0 || b[4] > W || b[3] >= b[4])
             return fail(W2L_EINVAL, "box %d = (frame %d, y %d:%d, x %d:%d) is empty or outside the %d frames of %dx%d", n, b[0], b[1], b[2], b[3], b[4], F, H, W);
     }
-    if (ctx->box_cap < N) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->boxes_dev) cudaFree(ctx->boxes_dev);
-        void* p = nullptr;
-        CKR(dev_alloc(&p, (size_t)N * 5 * 4));
-        ctx->boxes_dev = (int*)p; ctx->box_cap = N;
-    }
+    CKR(ctx->boxes_dev.grow(ctx, (size_t)N * 5 * 4));
     CK(cudaMemcpyAsync(ctx->boxes_dev, boxes, (size_t)N * 5 * 4, cudaMemcpyHostToDevice, st));
     return W2L_OK;
 }
@@ -408,15 +364,8 @@ int w2l_lipsync_frames_u8(w2l_ctx* ctx, const float* mel, const uint8_t* frames,
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
     const size_t cb = (size_t)N * 96 * 96 * 3;
-    if (ctx->crop_cap < cb) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->crops_dev) cudaFree(ctx->crops_dev);
-        if (ctx->preds_dev) cudaFree(ctx->preds_dev);
-        void* p = nullptr;
-        CKR(dev_alloc(&p, cb)); ctx->crops_dev = (uint8_t*)p;
-        CKR(dev_alloc(&p, cb)); ctx->preds_dev = (uint8_t*)p;
-        ctx->crop_cap = cb;
-    }
+    CKR(ctx->crops_dev.grow(ctx, cb));
+    CKR(ctx->preds_dev.grow(ctx, cb));
     CKR(w2l_crop_resize_u8(ctx, frames, F, H, W, boxes_host, N, ctx->crops_dev, stream));
     CKR(w2l_generator_forward_u8(ctx, mel, ctx->crops_dev, ctx->preds_dev, N, stream));
     const long long total = (long long)N * H * W;
@@ -477,14 +426,7 @@ static int train_batch_args(w2l_ctx* ctx, const uint8_t* frames, int64_t n_frame
 }
 
 static int upload_samples(w2l_ctx* ctx, const int32_t* s, size_t n, cudaStream_t st) {
-    if (ctx->sample_cap < n) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->samples_dev) cudaFree(ctx->samples_dev);
-        ctx->samples_dev = nullptr; ctx->sample_cap = 0;
-        void* p = nullptr;
-        CKR(dev_alloc(&p, n * 4));
-        ctx->samples_dev = (int*)p; ctx->sample_cap = n;
-    }
+    CKR(ctx->samples_dev.grow(ctx, n * 4));
     CK(cudaMemcpyAsync(ctx->samples_dev, s, n * 4, cudaMemcpyHostToDevice, st));
     return W2L_OK;
 }
@@ -612,23 +554,12 @@ int w2l_syncnet_forward_frames(w2l_ctx* ctx, const float* mel, const float* fram
     return run_plan(ctx, pl, mel, frames, a_emb, v_emb, (cudaStream_t)stream);
 }
 
-static int ensure_scratch(w2l_ctx* ctx, size_t bytes) {
-    if (ctx->scratch_bytes >= bytes) return W2L_OK;
-    CK(cudaDeviceSynchronize());
-    if (ctx->scratch) cudaFree(ctx->scratch);
-    ctx->scratch = nullptr; ctx->scratch_bytes = 0;
-    void* p = nullptr;
-    CKR(dev_alloc(&p, bytes));
-    ctx->scratch = (float*)p; ctx->scratch_bytes = bytes;
-    return W2L_OK;
-}
-
 int w2l_cosine_bce_loss(w2l_ctx* ctx, const float* a_emb, const float* v_emb, const float* y, int B, int D, float* loss, void* stream) {
     if (!ctx || !a_emb || !v_emb || !loss) return fail(W2L_EINVAL, "null argument");
     if (B <= 0 || D <= 0) return fail(W2L_EINVAL, "bad shape B=%d D=%d", B, D);
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    CKR(ensure_scratch(ctx, (size_t)std::max(B, 4096) * 4));
+    CKR(ctx->scratch.grow(ctx, (size_t)std::max(B, 4096) * 4));
     cosine_bce_terms_kernel<<<(B + 3) / 4, 128, 0, st>>>(a_emb, v_emb, y, ctx->scratch, B, D);
     sum_scale_kernel<<<1, 1024, 0, st>>>(ctx->scratch, loss, B, 1.0f / (float)B);
     ctx->launches += 2;
@@ -643,7 +574,7 @@ int w2l_l1_loss(w2l_ctx* ctx, const float* x, const float* y, int64_t n, float* 
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
     const int blocks = (int)std::min<long long>(std::max<long long>((n / 4 + 255) / 256, 1), (long long)ctx->num_sms * 8);
-    CKR(ensure_scratch(ctx, (size_t)std::max(blocks, 4096) * 4));
+    CKR(ctx->scratch.grow(ctx, (size_t)std::max(blocks, 4096) * 4));
     l1_partial_kernel<<<blocks, 256, 0, st>>>(x, y, ctx->scratch, (long long)n);
     sum_scale_kernel<<<1, 1024, 0, st>>>(ctx->scratch, loss, blocks, (float)(1.0 / (double)n));
     ctx->launches += 2;
@@ -691,41 +622,34 @@ int w2l_conv_block_forward(w2l_ctx* ctx, const w2l_layer_info* spec, const float
     CKR(block_from_info(spec, name.empty() ? "block" : name.c_str(), N, H, W, &L, &Ho, &Wo));
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    // a private one-block "network"; a residual is read from the block input, which then stays in the plain NHWC layout
+    ctx->last_block_kernels.clear();
+    // a private one-block "network" and plan, released on return; a residual is read from the block input, which then
+    // stays in the plain NHWC layout
     NetW scratch;
     scratch.layers.resize(1);
-    int r = load_layer(ctx, &scratch.layers[0], L, weight, bias, bn_w, bn_b, bn_m, bn_v, H == 1 && W == 1,
-                       ctx->use_fold && !L.residual, nullptr, st);
-    Plan pl;
+    CKR(load_layer(ctx, &scratch.layers[0], L, weight, bias, bn_w, bn_b, bn_m, bn_v, H == 1 && W == 1,
+                   ctx->use_fold && !L.residual, nullptr, st));
+    Plan pl(ctx);
     pl.net = W2L_NET_DISC; pl.N = N; pl.B = N; pl.T = 0;
     pl.x2 = ctx->x2;
     Act in, out;
-    if (r == W2L_OK) r = plan_input_act(&pl, &in, N, H, W, L.cin, scratch.layers[0], L);
-    if (r == W2L_OK) r = plan_act(&pl, &out, N, Ho, Wo, L.cout);
-    ctx->last_block_kernels.clear();
-    if (r == W2L_OK) {
-        add_ingest(&pl, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, in);
-        r = emit_block(ctx, &pl, scratch, 0, L, in, out, L.residual ? &in : nullptr);
-        if (r == W2L_OK) {
-            for (const Op& op : pl.ops)
-                if (op.type == OP_CONV) { ctx->last_block_kernels.emplace_back(); op_kernel_info(ctx, op, &ctx->last_block_kernels.back()); }
-            Plan* lp = ctx->last_plan[W2L_NET_DISC];
-            r = run_plan(ctx, &pl, x, nullptr, nullptr, nullptr, st);  // (pl.net only labels the plan)
-            ctx->last_plan[W2L_NET_DISC] = lp;
-        }
-    }
-    if (r == W2L_OK) {
-        const long long total = (long long)N * L.cout * Ho * Wo;
-        const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
-        if (ctx->bf16) export_kernel<true><<<blocks, 256, 0, st>>>(out.base, y, N, Ho, Wo, L.cout, out.Cs, 0, out.lo_off);
-        else export_kernel<false><<<blocks, 256, 0, st>>>(out.base, y, N, Ho, Wo, L.cout, out.Cs, 0, out.lo_off);
-        ctx->launches++;
-        cudaError_t e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) r = fail(W2L_ECUDA, "conv block failed: %s", cudaGetErrorString(e));
-    }
-    free_plan(&pl);
-    free_layer(scratch.layers[0]);
-    return r;
+    CKR(plan_input_act(&pl, &in, N, H, W, L.cin, scratch.layers[0], L));
+    CKR(plan_act(&pl, &out, N, Ho, Wo, L.cout));
+    add_ingest(&pl, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, in);
+    CKR(emit_block(ctx, &pl, scratch, 0, L, in, out, L.residual ? &in : nullptr));
+    for (const Op& op : pl.ops)
+        if (op.type == OP_CONV) { ctx->last_block_kernels.emplace_back(); op_kernel_info(ctx, op, &ctx->last_block_kernels.back()); }
+    Plan* lp = ctx->last_plan[W2L_NET_DISC];
+    const int r = run_plan(ctx, &pl, x, nullptr, nullptr, nullptr, st);  // (pl.net only labels the plan)
+    ctx->last_plan[W2L_NET_DISC] = lp;
+    CKR(r);
+    const long long total = (long long)N * L.cout * Ho * Wo;
+    const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
+    if (ctx->bf16) export_kernel<true><<<blocks, 256, 0, st>>>(out.base, y, N, Ho, Wo, L.cout, out.Cs, 0, out.lo_off);
+    else export_kernel<false><<<blocks, 256, 0, st>>>(out.base, y, N, Ho, Wo, L.cout, out.Cs, 0, out.lo_off);
+    ctx->launches++;
+    CK(cudaStreamSynchronize(st));
+    return W2L_OK;
 }
 
 int w2l_debug_kernel_table(int cap, w2l_kernel_info* out) {
@@ -808,10 +732,10 @@ int w2l_melspectrogram_host(w2l_ctx* ctx, const float* wav_h, int64_t n_samples,
     DeviceGuard g(ctx->device);
     CKR(host_drain(ctx, 0));  // the staging buffers below are slot 0 of the asynchronous host pipeline
     const int64_t F = w2l_mel_num_frames(n_samples);
-    CKR(ensure_stage(ctx, 0, (size_t)n_samples * 4));
-    CKR(ensure_stage(ctx, 4, (size_t)F * MEL_BANDS * 4));
+    CKR(ctx->stage[0].grow(ctx, (size_t)n_samples * 4));
+    CKR(ctx->stage[4].grow(ctx, (size_t)F * MEL_BANDS * 4));
     CK(cudaMemcpyAsync(ctx->stage[0], wav_h, (size_t)n_samples * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CKR(w2l_melspectrogram(ctx, (const float*)ctx->stage[0], n_samples, (float*)ctx->stage[4], ctx->stream));
+    CKR(w2l_melspectrogram(ctx, (const float*)ctx->stage[0].p, n_samples, (float*)ctx->stage[4].p, ctx->stream));
     CK(cudaMemcpyAsync(mel_h, ctx->stage[4], (size_t)F * MEL_BANDS * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return W2L_OK;
@@ -864,15 +788,11 @@ int w2l_train_bind(w2l_ctx* ctx, int net, int n_tensors, const char* const* name
     CK(cudaDeviceSynchronize());
     // plans bake the bound pointers: drop the ones of this net
     for (auto it = ts->plans.begin(); it != ts->plans.end();) {
-        if (it->second->net == net) { free_train_plan(it->second.get()); it = ts->plans.erase(it); }
+        if (it->second->net == net) it = ts->plans.erase(it);
         else ++it;
     }
     ts->last[net] = nullptr;
-    AdamSlot& a = ts->adam[net];
-    for (float* p : a.m) cudaFree(p);
-    for (float* p : a.v) cudaFree(p);
-    if (a.dev) cudaFree(a.dev);
-    a = AdamSlot();
+    ts->adam[net] = AdamSlot();
     ts->bound[net].clear();
     for (int i = 0; i < n_tensors; ++i) {
         std::string nm = names[i];
@@ -965,9 +885,9 @@ int w2l_comm_init(w2l_ctx* ctx, const char* id128, int rank, int world) {
     memcpy(id.bytes, id128, 128);
     const int rc = init(&ts->comm, world, id, rank);
     if (rc != 0) { ts->comm = nullptr; return fail(W2L_ECUDA, "ncclCommInitRank failed: %s", ts->err_string ? ts->err_string(rc) : "?"); }
-    CK(cudaStreamCreateWithFlags(&ts->s_comm, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&ts->ev_bucket, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&ts->ev_comm, cudaEventDisableTiming));
+    CKR(ts->s_comm.create());
+    CKR(ts->ev_bucket.create());
+    CKR(ts->ev_comm.create());
     return W2L_OK;
 }
 
@@ -1192,7 +1112,7 @@ int w2l_adam_state(w2l_ctx* ctx, int net, int direction, int n, const char* cons
 /* generator output of the last fused step (B,3,T,96,96) fp32, device pointer owned by the context (tests / logging) */
 int w2l_train_last_output(w2l_ctx* ctx, float* out, int64_t n, void* stream) {
     if (!ctx || !out || !ctx->train || !ctx->train->g_buf) return fail(W2L_ESTATE, "no fused training step has run");
-    if (n <= 0 || (size_t)n > ctx->train->g_cap) return fail(W2L_EINVAL, "bad element count");
+    if (n <= 0 || (size_t)n > ctx->train->g_buf.cap / 4) return fail(W2L_EINVAL, "bad element count");
     DeviceGuard g(ctx->device);
     CK(cudaMemcpyAsync(out, ctx->train->g_buf, (size_t)n * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return W2L_OK;
@@ -1213,9 +1133,9 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
     if (!tp) return fail(W2L_ESTATE, "no training forward has run for net %d", net);
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
+    Event e0, e1;
+    CKR(e0.create(cudaEventDefault));
+    CKR(e1.create(cudaEventDefault));
     int k = 0;
     auto timed = [&](const std::string& name, double flops, const std::function<int()>& fn) -> int {
         if (k >= cap) return W2L_OK;
@@ -1232,37 +1152,27 @@ int w2l_train_profile(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, 
         ++k;
         return W2L_OK;
     };
-    int r = W2L_OK;
     for (TBlock& b : tp->blocks) {
         double f = 0;
         for (size_t i = b.fwd0; i < b.fwd1; ++i) f += tp->pl.ops[i].flops;
         // forward conv only, then the statistics + normalise passes (running averages untouched)
-        r = timed(b.L.name + " fwd", f, [&]() -> int { for (size_t i = b.fwd0; i < b.fwd1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; });
-        if (r != W2L_OK) break;
+        CKR(timed(b.L.name + " fwd", f, [&]() -> int { for (size_t i = b.fwd0; i < b.fwd1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; }));
         if (b.bn) {
             TBlock c = b; c.fwd0 = c.fwd1 = 0;
-            r = timed(b.L.name + " bn", 0, [&]() -> int { return block_forward(ctx, tp, c, false, st); });
-            if (r != W2L_OK) break;
+            CKR(timed(b.L.name + " bn", 0, [&]() -> int { return block_forward(ctx, tp, c, false, st); }));
         }
         {
             TBlock c = b; c.dg0 = c.dg1 = 0; c.wg.on = false;
-            r = timed(b.L.name + " bwd_bn", 0, [&]() -> int { return block_backward(ctx, tp, c, false, false, true, st); });
-            if (r != W2L_OK) break;
+            CKR(timed(b.L.name + " bwd_bn", 0, [&]() -> int { return block_backward(ctx, tp, c, false, false, true, st); }));
         }
         if (b.dg1 > b.dg0) {
             double fd = 0;
             for (size_t i = b.dg0; i < b.dg1; ++i) fd += tp->pl.ops[i].flops;
-            r = timed(b.L.name + " dgrad", fd, [&]() -> int { for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; });
-            if (r != W2L_OK) break;
+            CKR(timed(b.L.name + " dgrad", fd, [&]() -> int { for (size_t i = b.dg0; i < b.dg1; ++i) CKR(launch_conv(ctx, tp->pl.ops[i], st, false)); return W2L_OK; }));
         }
-        if (b.wg.on) {
-            r = timed(b.L.name + " wgrad", b.wg.flops, [&]() -> int { return launch_wgrad(ctx, tp, b, false, st, false); });
-            if (r != W2L_OK) break;
-        }
+        if (b.wg.on) CKR(timed(b.L.name + " wgrad", b.wg.flops, [&]() -> int { return launch_wgrad(ctx, tp, b, false, st, false); }));
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    return r == W2L_OK ? k : r;
+    return k;
 }
 
 /* One block, train mode, forward + backward (the operator-level entry of the per-geometry gradient tests):
@@ -1278,10 +1188,16 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
     TrainState* ts = train_state(ctx);
+    ts->last_block_info.clear();
     CKR(ensure_train_scratch(ctx, 1, 1));
     const int slot = W2L_NET_DISC;
-    std::map<std::string, ParamRef> saved;
-    saved.swap(ts->bound[slot]);
+    // the block's tensors are bound in the discriminator's slot for this call; the caller's binding comes back on return
+    struct Rebind {
+        std::map<std::string, ParamRef>& live;
+        std::map<std::string, ParamRef> saved;
+        explicit Rebind(std::map<std::string, ParamRef>& m) : live(m) { saved.swap(live); }
+        ~Rebind() { live.swap(saved); }
+    } rebind(ts->bound[slot]);
     const long long wn = (long long)L.cin * L.cout * L.kh * L.kw;
     ts->bound[slot]["block.conv_block.0.weight"] = ParamRef{weight, dw, wn};
     ts->bound[slot]["block.conv_block.0.bias"] = ParamRef{bias, db, L.cout};
@@ -1292,51 +1208,43 @@ int w2l_conv_block_train(w2l_ctx* ctx, const w2l_layer_info* spec, const float* 
         if (bn_mean) ts->bound[slot]["block.conv_block.1.running_mean"] = ParamRef{bn_mean, nullptr, L.cout};
         if (bn_var) ts->bound[slot]["block.conv_block.1.running_var"] = ParamRef{bn_var, nullptr, L.cout};
     }
-    TrainPlan tp;
+    TrainPlan tp(ctx);   // released on return, before the binding
     tp.net = slot; tp.N = N; tp.B = N; tp.T = 0;
     Act xin, dxin, yv, dyv, none;
     size_t ws_need[2] = {0, 0};
-    int r = tp_act(&tp, &xin, N, H, W, round_up(L.cin, 16));
-    if (r == W2L_OK) r = tp_act(&tp, &dxin, N, H, W, round_up(L.cin, 16));
-    if (r == W2L_OK) r = tp_act(&tp, &yv, N, Ho, Wo, L.cout);
-    if (r == W2L_OK) r = tp_act(&tp, &dyv, N, Ho, Wo, L.cout);
-    if (r == W2L_OK) {
-        add_train_ingest(&tp, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, xin);
-        add_train_ingest(&tp, "ingest.dy", IngestSpec{1, N, L.cout, (long long)L.cout * Ho * Wo, (long long)Ho * Wo, 0, 0, Wo}, dyv);
-        r = add_train_block(ctx, &tp, slot, 0, L, xin, yv, dyv, dx ? dxin : none, none, dw != nullptr,
-                            L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, ws_need);
-    }
-    if (r == W2L_OK && ws_need[0]) { void* p = nullptr; r = plan_alloc(&tp.pl, &p, ws_need[0]); tp.wg_ws[0] = (float*)p; }
-    if (r == W2L_OK) {
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) r = fail(W2L_ECUDA, "plan build failed: %s", cudaGetErrorString(e));
-    }
-    if (r == W2L_OK) r = repack_weights(ctx, &tp, st);
-    if (r == W2L_OK) r = launch_ingest(ctx, tp.pl.ops[tp.ingest[0]], x, st);
-    if (r == W2L_OK) r = block_forward(ctx, &tp, tp.blocks[0], true, st);
-    if (r == W2L_OK) {
+    CKR(tp_act(&tp, &xin, N, H, W, round_up(L.cin, 16)));
+    CKR(tp_act(&tp, &dxin, N, H, W, round_up(L.cin, 16)));
+    CKR(tp_act(&tp, &yv, N, Ho, Wo, L.cout));
+    CKR(tp_act(&tp, &dyv, N, Ho, Wo, L.cout));
+    add_train_ingest(&tp, "ingest.x", IngestSpec{0, N, L.cin, (long long)L.cin * H * W, (long long)H * W, 0, 0, W}, xin);
+    add_train_ingest(&tp, "ingest.dy", IngestSpec{1, N, L.cout, (long long)L.cout * Ho * Wo, (long long)Ho * Wo, 0, 0, Wo}, dyv);
+    CKR(add_train_block(ctx, &tp, slot, 0, L, xin, yv, dyv, dx ? dxin : none, none, dw != nullptr,
+                        L.kind == W2L_BLOCK_CONVT_BN_RELU && H == 1 && W == 1, ws_need));
+    if (ws_need[0]) CKR(plan_alloc(&tp.pl, &tp.wg_ws[0], ws_need[0]));
+    CK(cudaDeviceSynchronize());
+    CKR(repack_weights(ctx, &tp, st));
+    CKR(launch_ingest(ctx, tp.pl.ops[tp.ingest[0]], x, st));
+    CKR(block_forward(ctx, &tp, tp.blocks[0], true, st));
+    {
         const long long total = (long long)N * L.cout * Ho * Wo;
         const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
         export_kernel<true><<<blocks, 256, 0, st>>>(yv.base, y, N, Ho, Wo, L.cout, yv.Cs, 0, 0);
         ctx->launches++;
     }
-    if (r == W2L_OK && dy) {
-        r = launch_ingest(ctx, tp.pl.ops[tp.ingest[1]], dy, st);
-        if (r == W2L_OK) r = block_backward(ctx, &tp, tp.blocks[0], dw != nullptr, false, true, st);
-        if (r == W2L_OK && dx) {
+    if (dy) {
+        CKR(launch_ingest(ctx, tp.pl.ops[tp.ingest[1]], dy, st));
+        CKR(block_backward(ctx, &tp, tp.blocks[0], dw != nullptr, false, true, st));
+        if (dx) {
             const long long total = (long long)N * L.cin * H * W;
             const int blocks = (int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16);
             export_grad_kernel<true><<<blocks, 256, 0, st>>>(dxin.ptr(), dxin.Cs, dx, N, H, W, L.cin);
             ctx->launches++;
         }
     }
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (r == W2L_OK && e != cudaSuccess) r = fail(W2L_ECUDA, "conv block train failed: %s", cudaGetErrorString(e));
-    ts->last_block_info.clear();
-    if (r == W2L_OK) { ts->last_block_info.emplace_back(); train_block_info(ctx, &tp, tp.blocks[0], &ts->last_block_info.back()); }
-    free_train_plan(&tp);
-    ts->bound[slot].swap(saved);
-    return r;
+    CK(cudaStreamSynchronize(st));
+    ts->last_block_info.emplace_back();
+    train_block_info(ctx, &tp, tp.blocks[0], &ts->last_block_info.back());
+    return W2L_OK;
 }
 
 int w2l_debug_train_blocks(w2l_ctx* ctx, int net, int cap, w2l_train_block_info* out) {
@@ -1403,13 +1311,7 @@ int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* o
 
 int64_t w2l_launch_count(const w2l_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
-int64_t w2l_device_bytes(const w2l_ctx* ctx) {
-    if (!ctx) return 0;
-    size_t b = ctx->weight_bytes;
-    for (auto& kv : ctx->plans) b += kv.second->bytes;
-    for (int i = 0; i < 6; ++i) b += ctx->stage_bytes[i];
-    return (int64_t)b;
-}
+int64_t w2l_device_bytes(const w2l_ctx* ctx) { return ctx ? (int64_t)ctx->device_bytes : 0; }
 
 int w2l_profile_plan(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, double* flop_out, char (*names_out)[64], void* stream) {
     if (!ctx || net < 0 || net > 3 || iters <= 0) return fail(W2L_EINVAL, "bad argument");
@@ -1417,41 +1319,37 @@ int w2l_profile_plan(w2l_ctx* ctx, int net, int iters, int cap, float* ms_out, d
     if (!pl) return fail(W2L_ESTATE, "no forward has run for net %d", net);
     DeviceGuard g(ctx->device);
     cudaStream_t st = (cudaStream_t)stream;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
+    Event e0, e1;
+    CKR(e0.create(cudaEventDefault));
+    CKR(e1.create(cudaEventDefault));
     // Cold-cache timing: the 126 MB L2 is flushed (a 256 MB buffer is overwritten) before EVERY timed launch, so that layers
     // whose tensors fit the L2 are not timed warm (the timing rule: flush L2 between timed iterations).
     const size_t flush_bytes = (size_t)256 << 20;
-    void* flush = nullptr;
-    if (cudaMalloc(&flush, flush_bytes) != cudaSuccess) { cudaGetLastError(); flush = nullptr; }
+    DevMem<> flush;
+    if (flush.grow(ctx, flush_bytes) != W2L_OK) g_err.clear();   // without it the timings are warm-cache
     int k = 0;
-    int r = W2L_OK;
     for (Op& op : pl->ops) {
         if (op.type != OP_CONV || k >= cap) continue;
         if (op.head && op.cp.ep.head_out == nullptr && op.pp.ep.head_out == nullptr && op.cp.ep.head_out_u8 == nullptr) continue;
-        if ((r = launch_conv(ctx, op, st, false)) != W2L_OK) break;  // warm the instruction cache / attributes
+        CKR(launch_conv(ctx, op, st, false));  // warm the instruction cache / attributes
         float total = 0.0f;
-        for (int i = 0; i < iters && r == W2L_OK; ++i) {
+        for (int i = 0; i < iters; ++i) {
             if (flush) cudaMemsetAsync(flush, i, flush_bytes, st);
             cudaEventRecord(e0, st);
-            r = launch_conv(ctx, op, st, false);
+            const int r = launch_conv(ctx, op, st, false);
             cudaEventRecord(e1, st);
-            if (cudaEventSynchronize(e1) != cudaSuccess) { r = fail(W2L_ECUDA, "profile: %s", cudaGetErrorString(cudaGetLastError())); break; }
+            if (cudaEventSynchronize(e1) != cudaSuccess) return fail(W2L_ECUDA, "profile: %s", cudaGetErrorString(cudaGetLastError()));
+            CKR(r);
             float ms = 0;
             cudaEventElapsedTime(&ms, e0, e1);
             total += ms;
         }
-        if (r != W2L_OK) break;
         if (ms_out) ms_out[k] = total / iters;
         if (flop_out) flop_out[k] = op.flops;
         if (names_out) snprintf(names_out[k], 64, "%s", op.name.c_str());
         ++k;
     }
-    if (flush) cudaFree(flush);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    return r == W2L_OK ? k : r;
+    return k;
 }
 
 }  // extern "C"
