@@ -51,8 +51,6 @@ constexpr int kMaxTaps = 49;              // filter taps of one launch
 constexpr int kMaxSteps = 3 * kMaxTaps;   // K-loop entries: x3 in the split-operand (fp32-faithful) precision mode
 constexpr int kSmemExtra = 2048;         // 1024 alignment slack + barriers
 constexpr int kSmemMax = 227 * 1024;     // dynamic shared memory limit per CTA on sm_90
-// patch kernels: weights + patch ring + staging; the two consumer warpgroups' transpose buffers and the barriers come on top
-constexpr int kSmemBudget = kSmemMax - kSmemExtra - 2 * xbuf_bytes<32>();
 
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_LRELU = 2 };
 
@@ -206,9 +204,10 @@ struct ConvCfg {
 __device__ int g_f16_overflow = 0;
 
 // `live` = the value belongs to a real output pixel.  (GEMM rows beyond a partial tile box are computed from stale shared
-// memory — any bit pattern, NaN included — and never stored; they must not raise the flag.)
+// memory — any bit pattern, NaN included — and never stored; they must not raise the flag.)  pack2_live takes it per
+// half: bit 15 = a is live, bit 31 = b is live.
 template <bool kBF16>
-__device__ __forceinline__ uint32_t pack2(float a, float b, bool live = true) {
+__device__ __forceinline__ uint32_t pack2_live(float a, float b, uint32_t live_bits) {
     if constexpr (kBF16) {
         __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
         return *reinterpret_cast<uint32_t*>(&h);
@@ -216,9 +215,13 @@ __device__ __forceinline__ uint32_t pack2(float a, float b, bool live = true) {
         __half2 h = __floats2half2_rn(a, b);
         const uint32_t u = *reinterpret_cast<uint32_t*>(&h);
         // exponent field all ones (inf / NaN) in either half: adding 0x0400 to the magnitude bits carries into bit 15
-        if (live && (((u & 0x7FFF7FFFu) + 0x04000400u) & 0x80008000u)) g_f16_overflow = 1;
+        if (((u & 0x7FFF7FFFu) + 0x04000400u) & live_bits) g_f16_overflow = 1;
         return u;
     }
+}
+template <bool kBF16>
+__device__ __forceinline__ uint32_t pack2(float a, float b, bool live = true) {
+    return pack2_live<kBF16>(a, b, live ? 0x80008000u : 0u);
 }
 template <bool kBF16>
 __device__ __forceinline__ float2 unpack2(uint32_t u) {

@@ -28,6 +28,17 @@
 //   * results are staged in swizzled shared memory and written with ONE TMA tensor store per tile (which also
 //     clips ragged edges), instead of 128 threads x 8 scattered 16-byte stores;
 //   * scale/shift/head weights come from the constant bank (kernel params).
+//
+// Channel-major form (BN = 64, BK = 64, no head: the 64 -> 64 residual blocks).  With pixels on M and 64 channels on N,
+// every m64n64k16 reads 2 KB of A and 2 KB of B from shared memory per 64 tensor clocks, which is the SM's whole
+// shared-memory bandwidth before the epilogue touches it.  This form swaps the operand roles: the 64 output channels
+// are M (the resident weight slab [tap][cout][cin] is already the K-major A operand) and a tile of 8 x 32 = 256 pixels
+// is N (the haloed 10 x 34 patch is the K-major B operand, tap t at patch + tap_row[t] rows, one 8-row group per output
+// row).  One m64n256k16 reads 2 + 8 KB per 128 clocks.  The epilogue works on the accumulator fragment (rows =
+// channels, so a thread needs the scale / shift of 2 channels): the residual comes from the patch centre by
+// ldmatrix.trans, the output goes to a pixel-major swizzled staging tile by stmatrix.trans and leaves by one TMA store.
+// A warpgroup holds 64 x 256 fp32 accumulators (128 registers per thread): setmaxnreg moves registers from the
+// producer warpgroup to the consumers.
 #pragma once
 
 #include "conv_igemm.cuh"
@@ -35,6 +46,8 @@
 namespace w2l {
 
 constexpr int kPatchTileW = 8, kPatchTileH = 16;  // output tile (pixels)
+constexpr int kChTileH = 32;                       // output tile height of the channel-major form (8 x 32 pixels)
+__host__ __device__ constexpr bool patch_chmajor(int BN, int BK, bool head) { return BN == 64 && BK == 64 && !head; }
 constexpr int kPatchThreads = 384;       // warps: 0 TMA, 1 barrier init, 2-3 idle, 4-7 consumer A, 8-11 consumer B
 constexpr int kPatchMaxTaps = 9;
 constexpr int kPatchMaxStages = 8;
@@ -42,7 +55,7 @@ constexpr int kPatchMaxStages = 8;
 struct alignas(64) PatchParams {
     CUtensorMap tmA;  // activations (C, W, H, N), box (BK, PW, PH, 1)
     CUtensorMap tmB;  // weights (Cin_pad, Cout_pad, taps), box (BK, BN, 1)
-    CUtensorMap tmO;  // output channel slice (BN, Wl, Hl, N) with the launch's pixel strides, box (BN, 8, 16, 1)
+    CUtensorMap tmO;  // output channel slice (BN, Wl, Hl, N) with the launch's pixel strides, box (BN, 8, tile height, 1)
     CUtensorMap tmO2; // optional second destination of the same tile (a dense zero-bordered copy for a folded consumer)
     int has_out2;
     int tiles_x, tiles_y;   // tiles per image
@@ -68,6 +81,8 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     constexpr int CW = BN < 32 ? BN : 32;
     static_assert(BN <= 64, "resident-weight variant is for narrow layers");
     static_assert(!kHead || BN == 32, "fused head expects the 32-channel output block");
+    constexpr bool kCM = patch_chmajor(BN, BK, kHead);
+    constexpr int kTileH = kCM ? kChTileH : kPatchTileH;
 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_raw_u32 = smem_u32(smem_raw);
@@ -78,9 +93,9 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     const uint32_t w_base = smem_base;
     const uint32_t a_base = w_base + static_cast<uint32_t>(ntaps * kc) * kSlab;
     const uint32_t stg_base = a_base + static_cast<uint32_t>(stages * kc) * p.patch_stride;  // a stage = all chunks of one tile
-    constexpr uint32_t kStgBytes = ((kTileM * BN * 2 + 1023) / 1024) * 1024;                  // one staging tile per group
+    constexpr uint32_t kStgBytes = ((kPatchTileW * kTileH * BN * 2 + 1023) / 1024) * 1024;    // one staging tile per group
     const uint32_t xb_base = stg_base + 2u * kStgBytes;
-    const uint32_t bar_base = xb_base + 2u * xbuf_bytes<32>();
+    const uint32_t bar_base = xb_base + (kCM ? 0u : 2u * xbuf_bytes<32>());  // the channel-major form needs no transpose buffers
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kPatchMaxStages + s); };
     const uint32_t w_bar = bar_base + 8u * (2 * kPatchMaxStages);
@@ -108,9 +123,10 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     const int tiles_per_img = p.tiles_x * p.tiles_y;
     const int total_tiles = tiles_per_img * p.ep.N;
 
-    if (warp == 0) {
+    if (warp < 4) {
+        if constexpr (kCM) setmaxnreg_dec<kProducerRegs>();
         // =============================== TMA producer ===============================
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             mbar_arrive_expect_tx(w_bar, static_cast<uint32_t>(ntaps * kc) * kSlab);
             for (int tap = 0; tap < ntaps; ++tap)
                 for (int c = 0; c < kc; ++c)
@@ -125,11 +141,127 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
                 mbar_arrive_expect_tx(full_bar(stage), static_cast<uint32_t>(kc) * p.patch_bytes);
                 for (int c = 0; c < kc; ++c)
                     tma_load_4d(a_base + (stage * kc + c) * p.patch_stride, &p.tmA, full_bar(stage), c * BK,
-                                tx * kPatchTileW + p.ox, ty * kPatchTileH + p.oy, n);
+                                tx * kPatchTileW + p.ox, ty * kTileH + p.oy, n);
                 if (++stage == stages) { stage = 0; phase ^= 1u; }
             }
         }
-    } else if (warp >= 4) {
+    } else if constexpr (kCM) {
+        setmaxnreg_inc<kConsumerRegs>();
+        // ===== channel-major consumer warpgroups, alternating tiles: D[64 channels x 256 pixels] = W[64 x K] * patch[K x 256] =====
+        // Fragment of m64n256k16: warp q of the group holds channels c = 16q + lane/4 (acc[4j + 0..1]) and c + 8
+        // (acc[4j + 2..3]) at pixels 8j + 2(lane%4) + {0,1}, i.e. row j of the 8 x 32 tile, columns 2(lane%4) + {0,1}.
+        const int grp = (warp - 4) >> 2;
+        const int q = (warp - 4) & 3;
+        const int ch = 16 * q + (lane >> 2);
+        const float sc0 = p.cscale[ch], sh0 = p.cshift[ch], sc1 = p.cscale[ch + 8], sh1 = p.cshift[ch + 8];
+        const int px = 2 * (lane & 3);
+        const EpiParams& e = p.ep;
+        const uint32_t stg = stg_base + grp * kStgBytes;
+        const bool leader = (q == 0 && lane == 0);
+        const uint32_t bar_id = 1 + grp;
+        // ldmatrix / stmatrix .x4: lanes 8m .. 8m+7 address the 8 pixel rows of matrix m = (tile row 2i + m/2, 16-byte
+        // channel chunk 2q + m%2), which land in / come from the fragment registers of (row 2i + m/2, channel ch + 8(m%2))
+        const int lm_row = lane >> 4, lm_px = lane & 7;
+        const uint32_t lm_chunk = 16u * (2 * q + ((lane >> 3) & 1));
+        const uint32_t sbo_b = static_cast<uint32_t>(p.PW) * kRowBytes;
+        uint32_t tap_off[kPatchMaxTaps];
+#pragma unroll
+        for (int t = 0; t < kPatchMaxTaps; ++t) tap_off[t] = (t < ntaps ? p.tap_row[t] : 0) * kRowBytes;
+        mbar_wait(w_bar, 0);
+        float acc[128];
+        for (int it = grp;; it += 2) {
+            const int tile = blockIdx.x + it * gridDim.x;
+            if (tile >= total_tiles) break;
+            const int stage = it % stages;
+            const int n = tile / tiles_per_img;
+            const int r = tile - n * tiles_per_img;
+            const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
+
+            mbar_wait(full_bar(stage), static_cast<uint32_t>(it / stages) & 1u);
+            wg_fence();
+            for (int c = 0; c < kc; ++c) {
+                const uint32_t patch = a_base + (stage * kc + c) * p.patch_stride;
+#pragma unroll
+                for (int tap = 0; tap < kPatchMaxTaps; ++tap)
+                    if (tap < ntaps) {
+#pragma unroll
+                        for (int k = 0; k < BK / 16; ++k)  // 16 channels further along K = 32 bytes inside the swizzle atom
+                            wgmma_m64k16<256, kBF16>(acc, make_kmajor_desc<BK>(w_base + (tap * kc + c) * kSlab + 32u * k),
+                                                     wg_desc(patch + tap_off[tap] + 32u * k, 16, sbo_b, kRowBytes),
+                                                     (c | tap | k) != 0 ? 1u : 0u, 0);
+                    }
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_fence_regs<128>(acc);
+            if (p.res_row < 0 && lane == 0) mbar_arrive(empty_bar(stage));  // the MMAs were the patch's last readers
+
+            // folded BatchNorm, then the residual = this block's input = centre of the patch (pixel-major, swizzled by
+            // address bits as TMA wrote it), read transposed into the fragment layout
+            const uint32_t res_base = a_base + stage * kc * p.patch_stride;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float* a = acc + 8 * i + 4 * h;
+                    a[0] = fmaf(a[0], sc0, sh0); a[1] = fmaf(a[1], sc0, sh0);
+                    a[2] = fmaf(a[2], sc1, sh1); a[3] = fmaf(a[3], sc1, sh1);
+                }
+                if (p.res_row >= 0) {
+                    uint32_t ad = res_base + static_cast<uint32_t>(p.res_row + (2 * i + lm_row) * p.PW + lm_px) * kRowBytes + lm_chunk;
+                    ad ^= ((ad >> 7) & 7u) << 4;
+                    uint32_t rv[4];
+                    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+                                 : "=r"(rv[0]), "=r"(rv[1]), "=r"(rv[2]), "=r"(rv[3]) : "r"(ad));
+#pragma unroll
+                    for (int m = 0; m < 4; ++m) {
+                        const float2 v = unpack2<kBF16>(rv[m]);
+                        acc[8 * i + 2 * m] += v.x;
+                        acc[8 * i + 2 * m + 1] += v.y;
+                    }
+                }
+            }
+            if (p.res_row >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(stage));  // this warp is done with the patch
+            }
+            if (e.act == ACT_RELU) {
+#pragma unroll
+                for (int j = 0; j < 128; ++j) acc[j] = fmaxf(acc[j], 0.0f);
+            } else if (e.act == ACT_LRELU) {
+#pragma unroll
+                for (int j = 0; j < 128; ++j) acc[j] = acc[j] > 0.0f ? acc[j] : 0.01f * acc[j];
+            }
+            // stage the tile (pixel-major rows of 64 channels, 128-byte swizzle) by stmatrix.trans and TMA-store it; only
+            // pixels inside the image may raise the fp16 range flag
+            const int x = tx * kPatchTileW + px;
+            const uint32_t live_x = (x < e.Wout ? 0x8000u : 0u) | (x + 1 < e.Wout ? 0x80000000u : 0u);
+            const int rows_live = e.Hout - ty * kTileH;
+            if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the buffer
+            named_bar_sync(bar_id, 128);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                uint32_t ad = stg + static_cast<uint32_t>((2 * i + lm_row) * kPatchTileW + lm_px) * kRowBytes + lm_chunk;
+                ad ^= ((ad >> 7) & 7u) << 4;
+                const uint32_t l0 = 2 * i < rows_live ? live_x : 0u, l1 = 2 * i + 1 < rows_live ? live_x : 0u;
+                const uint32_t o0 = pack2_live<kBF16>(acc[8 * i + 0], acc[8 * i + 1], l0);
+                const uint32_t o1 = pack2_live<kBF16>(acc[8 * i + 2], acc[8 * i + 3], l0);
+                const uint32_t o2 = pack2_live<kBF16>(acc[8 * i + 4], acc[8 * i + 5], l1);
+                const uint32_t o3 = pack2_live<kBF16>(acc[8 * i + 6], acc[8 * i + 7], l1);
+                asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1,%2,%3,%4};"
+                             ::"r"(ad), "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
+            named_bar_sync(bar_id, 128);
+            if (leader) {
+                asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                             ::"l"(reinterpret_cast<uint64_t>(&p.tmO)), "r"(stg), "r"(0), "r"(tx * kPatchTileW), "r"(ty * kTileH), "r"(n)
+                             : "memory");
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        }
+        if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
+    } else {
         // ============ consumer warpgroups (MMA + epilogue), alternating tiles: group g takes tiles g, g+2, .. ============
         const int grp = (warp - 4) >> 2;
         const int q = (warp - 4) & 3;

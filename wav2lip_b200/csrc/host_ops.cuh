@@ -114,7 +114,10 @@ static int encode_w_map(w2l_ctx* ctx, CUtensorMap* tm, const PackedW& w, int BK,
 }
 
 // Few-channel stride-1 layers: one input patch per tile + resident weights (conv_patch.cuh)
-struct PatchGeom { int ox, oy, PW, PH, BK, patch_bytes, patch_stride, wbytes, stg_bytes, res_tap; };
+struct PatchGeom { int ox, oy, PW, PH, BK, TH, patch_bytes, patch_stride, wbytes, stg_bytes, xbuf_bytes, res_tap; };
+
+// weights + patch ring + staging; the transpose buffers of the row-per-thread form and the barriers come on top
+static int patch_smem_budget(const PatchGeom& g) { return kSmemMax - kSmemExtra - g.xbuf_bytes; }
 
 static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) {
     if (!ctx->use_patch) return false;
@@ -125,22 +128,26 @@ static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) 
     if (a.head && a.cout != 32) return false;
     if (a.Wl < kPatchTileW || a.Hl < kPatchTileW) return false;
     if (a.out.f32) return false;
-    const double tiles = (double)((a.Wl + kPatchTileW - 1) / kPatchTileW) * ((a.Hl + kPatchTileH - 1) / kPatchTileH);
-    if ((double)a.Wl * a.Hl / (tiles * kTileM) < 0.6) return false;
+    g->BK = pick_bk(w.cin_pad);
+    // the 64 -> 64 form runs channel-major on 8 x 32 tiles and needs no transpose buffers (conv_patch.cuh)
+    const bool chm = patch_chmajor(a.cout, g->BK, a.head);
+    g->TH = chm ? kChTileH : kPatchTileH;
+    g->xbuf_bytes = chm ? 0 : 2 * xbuf_bytes<32>();
+    const double tiles = (double)((a.Wl + kPatchTileW - 1) / kPatchTileW) * ((a.Hl + g->TH - 1) / g->TH);
+    if ((double)a.Wl * a.Hl / (tiles * kPatchTileW * g->TH) < 0.6) return false;
     int mnx = 127, mxx = -127, mny = 127, mxy = -127;
     for (int t = 0; t < w.ntaps; ++t) {
         mnx = std::min(mnx, (int)w.dx[t]); mxx = std::max(mxx, (int)w.dx[t]);
         mny = std::min(mny, (int)w.dy[t]); mxy = std::max(mxy, (int)w.dy[t]);
     }
     g->ox = mnx; g->oy = mny;
-    g->PW = kPatchTileW + (mxx - mnx); g->PH = kPatchTileH + (mxy - mny);
-    g->BK = pick_bk(w.cin_pad);
+    g->PW = kPatchTileW + (mxx - mnx); g->PH = g->TH + (mxy - mny);
     g->patch_bytes = g->PW * g->PH * g->BK * 2;
     g->patch_stride = (g->patch_bytes + 1023) / 1024 * 1024;
     g->wbytes = w.ntaps * w.cin_pad * a.cout * 2;
-    g->stg_bytes = 2 * ((kTileM * a.cout * 2 + 1023) / 1024 * 1024);  // the kernel always carves two staging tiles
+    g->stg_bytes = 2 * ((kPatchTileW * g->TH * a.cout * 2 + 1023) / 1024 * 1024);  // the kernel always carves two staging tiles
     if (g->PW > 256 || g->PH > 256) return false;
-    if (g->wbytes + g->stg_bytes + 2 * (w.cin_pad / g->BK) * g->patch_stride > kSmemBudget) return false;
+    if (g->wbytes + g->stg_bytes + 2 * (w.cin_pad / g->BK) * g->patch_stride > patch_smem_budget(*g)) return false;
     g->res_tap = -1;
     if (a.res) {
         // the patch kernel takes the residual from the input patch in shared memory: it must BE the block input
@@ -167,27 +174,27 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     CKR(encode_act_map(ctx, &h.tmA, a.in, BK, g.PW, g.PH, 1, 1, 1, a.name.c_str()));
     CKR(encode_w_map(ctx, &h.tmB, w, BK, BN, a.name.c_str()));
     h.tiles_x = (a.Wl + kPatchTileW - 1) / kPatchTileW;
-    h.tiles_y = (a.Hl + kPatchTileH - 1) / kPatchTileH;
+    h.tiles_y = (a.Hl + g.TH - 1) / g.TH;
     h.kc = w.cin_pad / BK;
     h.PW = g.PW; h.PH = g.PH; h.ox = g.ox; h.oy = g.oy;
     h.ntaps = w.ntaps;
     h.patch_bytes = g.patch_bytes; h.patch_stride = g.patch_stride;
     for (int t = 0; t < w.ntaps; ++t) h.tap_row[t] = (w.dy[t] - g.oy) * g.PW + (w.dx[t] - g.ox);
     // even: the two consumer warpgroups take alternate tiles, so each stage always goes to the same one
-    h.stages = std::min(kPatchMaxStages, (kSmemBudget - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride)) & ~1;
-    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + 2 * xbuf_bytes<32>() + kSmemExtra;
+    h.stages = std::min(kPatchMaxStages, (patch_smem_budget(g) - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride)) & ~1;
+    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + g.xbuf_bytes + kSmemExtra;
     if (op.dyn_smem > kSmemMax || h.stages < 2) return fail(W2L_EINVAL, "%s: patch kernel smem plan %d B / %d stages", a.name.c_str(), op.dyn_smem, h.stages);
     fill_epi(&h.ep, a);
     h.res_row = g.res_tap >= 0 ? h.tap_row[g.res_tap] : -1;
     if (!a.head) {
         // TMA-store view of the output: the BN-channel slice, with this launch's pixel strides (transposed-conv phases
-        // interleave), box = one 8 x 16 tile; out-of-range pixels of ragged tiles are clipped by the TMA unit
+        // interleave), box = one tile; out-of-range pixels of ragged tiles are clipped by the TMA unit
         EncodeTiledFn enc = get_encode_fn();
         const CUtensorMapDataType dt = ctx->bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
         const CUtensorMapSwizzle sw = BN == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : BN == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
         cuuint64_t dims[4] = {(cuuint64_t)BN, (cuuint64_t)a.Wl, (cuuint64_t)a.Hl, (cuuint64_t)a.in.N};
         cuuint64_t strides[3] = {(cuuint64_t)h.ep.out_sx * 2, (cuuint64_t)h.ep.out_sy * 2, (cuuint64_t)h.ep.out_sn * 2};
-        cuuint32_t box[4] = {(cuuint32_t)BN, (cuuint32_t)kPatchTileW, (cuuint32_t)kPatchTileH, 1};
+        cuuint32_t box[4] = {(cuuint32_t)BN, (cuuint32_t)kPatchTileW, (cuuint32_t)g.TH, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
         if (a.out.f32) return fail(W2L_EINVAL, "%s: patch kernel stores 16-bit outputs only", a.name.c_str());
         CUresult r = enc(&h.tmO, dt, 4, h.ep.out, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
