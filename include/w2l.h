@@ -255,7 +255,8 @@ int w2l_mel_basis_host(float* out_host);
 #define W2L_KFAM_PATCH        1   /* patch kernel with resident weights (conv_patch.cuh) */
 #define W2L_KFAM_CONVT_FUSED  2   /* fused 4-phase transposed conv (convt_fused.cuh) */
 typedef struct w2l_kernel_info {
-    char    name[64];   /* the op's plan label ("b [patch]", "b.ph01 [2M]", ...); empty in the table listing */
+    char    name[64];   /* the op's plan label ("b [patch]", "b.ph01 [2M]", "b [cm]", ...); in the table listing "[cm]" for
+                         * an instantiation that also has the channel-major form, else empty */
     int32_t family;     /* W2L_KFAM_* */
     int32_t bn, bk, mt, head, bf16, x2, tma_epi, fold;
     int32_t m_tiles, n_tiles, grid;

@@ -33,6 +33,11 @@
 //             read the boxes.  Direct mode (fp32 outputs, split-operand mode, fused generator head
 //             wav2lip.py:84-85): a shared-memory transpose (wgmma.cuh: acc_to_rows) makes thread = GEMM row =
 //             output pixel, then per-thread global accesses.
+//   Channel-major form (kCM, BN = 128, BK = 64): the operand roles swap.  The 128 output channels are M (warpgroup g takes
+//             weight rows 64g.. as the K-major A operand), a box of kCmPixels = 256 output pixels is N (the activation box,
+//             the K-major B operand of m64n256k16, shared by both warpgroups), so a tile reads 80 instead of 96 bytes of
+//             shared memory per tensor clock.  Both warpgroups consume every stage and run their epilogues together
+//             (chmajor_epilogue: residual by ldmatrix.trans from the staging box, stmatrix.trans, one TMA store each).
 //
 // Everything a launch needs is in ConvParams (a __grid_constant__), built once per plan on the host.
 #pragma once
@@ -175,17 +180,22 @@ __device__ __forceinline__ void wg_mma_tile(float (&acc)[2][BN / 2], uint32_t a,
 // Shared memory: the K-step ring, then one region per consumer warpgroup that holds either the staging boxes of the
 // staged epilogue (the full tile width, BN / kEW boxes) or the transpose buffer of the direct one (a launch uses one
 // epilogue form), then the barriers.
-template <int BN, int BK, int MT = 1>
+// Channel-major form (CM): the tile is BN = 128 channels x kCmPixels pixels, each consumer warpgroup owns one 64-channel half
+// and its staging box (64 channels x kCmPixels pixels); the ring stage holds the pixel box and the weight slab.
+constexpr int kCmPixels = 256;
+template <int BN, int BK, int MT = 1, bool kCM = false>
 struct ConvCfg {
-    static constexpr int kATile = kTileM * BK * 2;
+    static constexpr int kRowsA = kCM ? kCmPixels : kTileM;       // pixel rows of one A (activation) tile
+    static constexpr int kATile = kRowsA * BK * 2;
     static constexpr int kABytes = MT * kATile;
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kEW = BN < 64 ? BN : 64;                 // channels per epilogue box (one TMA box)
     static constexpr int kCW = BN < 32 ? BN : 32;                 // accumulator columns per transpose chunk (direct epilogue)
-    static constexpr int kPasses = BN / kEW;                      // epilogue boxes per tile
-    static constexpr int kBoxBytes = kTileM * kEW * 2;            // one staging box: 128 rows x kEW 16-bit channels
-    static constexpr int kGrpRaw = kPasses * kBoxBytes > xbuf_bytes<kCW>() ? kPasses * kBoxBytes : xbuf_bytes<kCW>();
+    static constexpr int kPasses = kCM ? 1 : BN / kEW;            // epilogue boxes per warpgroup and tile
+    static constexpr int kBoxBytes = kRowsA * kEW * 2;            // one staging box: kRowsA rows x kEW 16-bit channels
+    // CM always stages its epilogue (no transpose buffer)
+    static constexpr int kGrpRaw = (kCM || kPasses * kBoxBytes > xbuf_bytes<kCW>()) ? kPasses * kBoxBytes : xbuf_bytes<kCW>();
     static constexpr int kGrpBytes = (kGrpRaw + 1023) / 1024 * 1024;  // epilogue region of one consumer warpgroup
     static constexpr int kStagesRaw = (kSmemMax - kSmemExtra - 2 * kGrpBytes) / kStageBytes;
     static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
@@ -193,6 +203,7 @@ struct ConvCfg {
     static constexpr int kSmemBytes = kRingBytes + 2 * kGrpBytes + kSmemExtra;
     static constexpr int kThreads = 384;  // the producer warpgroup + two consumer warpgroups
     static_assert(BN <= 128, "a warpgroup holds at most 128 fp32 accumulator columns per row");
+    static_assert(!kCM || (BN == 128 && BK == 64 && MT == 1), "channel-major form: 128 channels, 128-byte K rows, one tile");
     static_assert(kBoxBytes % 1024 == 0, "staging boxes must keep the 1024-byte swizzle alignment");
     static_assert(kStages >= 2, "need a pipeline");
     static_assert(kSmemBytes <= kSmemMax, "shared-memory carve-up exceeds the per-CTA limit");
@@ -329,6 +340,86 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&
     }
 }
 
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// Epilogue of a channel-major tile (conv_patch_kernel<64, 64> and conv_igemm_kernel<128, 64, ., ., 1, true>): one
+// warpgroup's m64n256 accumulator, rows = 64 output channels, columns = 256 output pixels.  Fragment: warp q holds channels
+// 16q + lane/4 (acc[4j + 0..1], scale / shift sc0 / sh0) and that + 8 (acc[4j + 2..3], sc1 / sh1) at pixels
+// 8j + 2(lane%4) + {0,1}.  The staging tile `stg` is pixel-major: pixel p is row p of 128 bytes (64 16-bit channels,
+// 128-byte swizzle), exactly the box the TMA store `tmO` writes at (c0, c1, c2, c3).
+//   res       : 0 = no residual, else the address of residual pixel 0 in a pixel-major 128-byte-row tile whose pixel rows of
+//               8 are res_pitch rows apart (the staging tile itself when the residual was TMA-loaded into it, pitch 8);
+//               read by ldmatrix.trans straight into the fragment layout
+//   after_res : called by every thread once its residual reads are done (the patch kernel releases its ring slot there)
+//   live(j)   : pack2_live bits of the pixel pair of column chunk j (only pixels inside the image may raise the fp16 flag)
+// Every warp reads and writes only its own 32-byte channel stripe of the tiles; the named barrier bar_id orders the
+// warpgroup's stmatrix writes after the previous TMA store has read the staging tile, and the store after the writes.
+template <bool kBF16, typename AfterRes, typename Live>
+__device__ __forceinline__ void chmajor_epilogue(float (&acc)[128], float sc0, float sh0, float sc1, float sh1, int act,
+                                                 uint32_t res, int res_pitch, AfterRes&& after_res, Live&& live, uint32_t stg,
+                                                 uint32_t bar_id, bool leader, const CUtensorMap* tmO, int c0, int c1, int c2,
+                                                 int c3) {
+    constexpr uint32_t kRowB = 128;
+    const int lane = threadIdx.x & 31, q = (threadIdx.x >> 5) & 3;
+    // ldmatrix / stmatrix .x4: lanes 8m .. 8m+7 address the 8 pixels of matrix m = (pixels 8(2i + m/2) .., 16-byte channel
+    // chunk 2q + m%2), which land in / come from the fragment registers of (column chunk 2i + m/2, channel half m%2)
+    const int lm_row = lane >> 4, lm_px = lane & 7;
+    const uint32_t lm_chunk = 16u * (2 * q + ((lane >> 3) & 1));
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float* a = acc + 8 * i + 4 * h;
+            a[0] = fmaf(a[0], sc0, sh0); a[1] = fmaf(a[1], sc0, sh0);
+            a[2] = fmaf(a[2], sc1, sh1); a[3] = fmaf(a[3], sc1, sh1);
+        }
+        if (res != 0) {
+            uint32_t ad = res + static_cast<uint32_t>((2 * i + lm_row) * res_pitch + lm_px) * kRowB + lm_chunk;
+            ad ^= ((ad >> 7) & 7u) << 4;
+            uint32_t rv[4];
+            asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+                         : "=r"(rv[0]), "=r"(rv[1]), "=r"(rv[2]), "=r"(rv[3]) : "r"(ad));
+#pragma unroll
+            for (int m = 0; m < 4; ++m) {
+                const float2 v = unpack2<kBF16>(rv[m]);
+                acc[8 * i + 2 * m] += v.x;
+                acc[8 * i + 2 * m + 1] += v.y;
+            }
+        }
+    }
+    after_res();
+    if (act == ACT_RELU) {
+#pragma unroll
+        for (int j = 0; j < 128; ++j) acc[j] = fmaxf(acc[j], 0.0f);
+    } else if (act == ACT_LRELU) {
+#pragma unroll
+        for (int j = 0; j < 128; ++j) acc[j] = acc[j] > 0.0f ? acc[j] : 0.01f * acc[j];
+    }
+    if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the staging tile
+    named_bar_sync(bar_id, 128);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        uint32_t ad = stg + static_cast<uint32_t>((2 * i + lm_row) * 8 + lm_px) * kRowB + lm_chunk;
+        ad ^= ((ad >> 7) & 7u) << 4;
+        const uint32_t l0 = live(2 * i), l1 = live(2 * i + 1);
+        const uint32_t o0 = pack2_live<kBF16>(acc[8 * i + 0], acc[8 * i + 1], l0);
+        const uint32_t o1 = pack2_live<kBF16>(acc[8 * i + 2], acc[8 * i + 3], l0);
+        const uint32_t o2 = pack2_live<kBF16>(acc[8 * i + 4], acc[8 * i + 5], l1);
+        const uint32_t o3 = pack2_live<kBF16>(acc[8 * i + 6], acc[8 * i + 7], l1);
+        asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1,%2,%3,%4};"
+                     ::"r"(ad), "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
+    named_bar_sync(bar_id, 128);
+    if (leader) {
+        asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                     ::"l"(reinterpret_cast<uint64_t>(tmO)), "r"(stg), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                     : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
@@ -340,16 +431,15 @@ template <int kRegs>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 template <int kRegs>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
-template <int BN, int BK, bool kBF16, bool kHead, int MT = 1>
-__global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
+template <int BN, int BK, bool kBF16, bool kHead, int MT = 1, bool kCM = false>
+__global__ void __launch_bounds__(ConvCfg<BN, BK, MT, kCM>::kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
     pdl_launch_dependents();
-    using Cfg = ConvCfg<BN, BK, MT>;
+    using Cfg = ConvCfg<BN, BK, MT, kCM>;
     constexpr int kStages = Cfg::kStages;
     static_assert(!kHead || BN == 32, "fused head expects the 32-channel output block");
     static_assert(MT == 1 || MT == 2, "one or two M tiles per unit");
+    static_assert(!kCM || !kHead, "the channel-major form stages its epilogue");
 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_raw_u32 = smem_u32(smem_raw);
@@ -374,7 +464,7 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 4 * MT);  // one arrive per warp of the warpgroup(s) that consume the step
+            mbar_init(empty_bar(s), kCM ? 8 : 4 * MT);  // one arrive per warp of the warpgroup(s) that consume the step
         }
         for (int g = 0; g < 2; ++g) mbar_init(res_bar(g), 1);
         fence_barrier_init();
@@ -423,6 +513,94 @@ __global__ void __launch_bounds__(ConvCfg<BN, BK, MT>::kThreads, 1) conv_igemm_k
                 }
             }
         }
+    } else if constexpr (kCM) {
+        setmaxnreg_inc<kConsumerRegs>();
+        // ===== channel-major consumers: both warpgroups work on every tile of the CTA.  Warpgroup g computes
+        // D[64 channels x 256 pixels] = W[64 x K] * box[K x 256]: its 64-row half of the weight slab is the K-major A
+        // operand, the pixel box (rows = pixels, 8-row groups 1024 B apart) the K-major B operand of m64n256k16.  Each warp
+        // releases a ring stage once the step that read it has retired (8 arrivals per stage). =====
+        const int g = (warp - 4) >> 2;
+        const int q = (warp - 4) & 3;
+        const uint32_t bar_id = 1 + g;
+        const bool leader = (q == 0 && lane == 0);
+        const uint32_t stg = grp_base + g * Cfg::kGrpBytes;  // this warpgroup's staging box (64 channels x 256 pixels)
+        const bool has_res = p.ep.res != nullptr;
+        const int rows_valid = p.bw * p.bh * p.bn;
+        const int ch = 64 * g + 16 * q + (lane >> 2);         // fragment channels ch and ch + 8 of the tile
+        auto tile_origin = [&](int tile_, int* nt_, int* x0_, int* y0_, int* n0_) {
+            *nt_ = tile_ % p.n_tiles;
+            const int m_ = tile_ / p.n_tiles;
+            *x0_ = (m_ % p.tiles_x) * p.bw;
+            *y0_ = ((m_ / p.tiles_x) % p.tiles_y) * p.bh;
+            *n0_ = (m_ / (p.tiles_x * p.tiles_y)) * p.bn;
+        };
+        // leader: request the tile's residual half into the staging box (the previous store must have read it)
+        auto fetch_res = [&](int tile_) {
+            int nt_, x0_, y0_, n0_;
+            tile_origin(tile_, &nt_, &x0_, &y0_, &n0_);
+            mbar_arrive_expect_tx(res_bar(g), p.epi_box_bytes);
+            tma_load_4d(stg, &p.tmR, res_bar(g), nt_ * BN + 64 * g, x0_, y0_, n0_);
+        };
+        if (has_res && leader && static_cast<int>(blockIdx.x) < total_tiles) fetch_res(blockIdx.x);
+        float acc[128];
+        int stage = 0;
+        uint32_t phase = 0, rphase = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            int prev = -1;
+            for (int ks = 0; ks < k_steps; ++ks) {
+                mbar_wait(full_bar(stage), phase);
+                const uint32_t box = smem_base + stage * Cfg::kStageBytes;
+                const uint32_t wts = box + Cfg::kABytes + g * (64 * BK * 2);
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)  // 16 elements further along K = 32 bytes inside the swizzle atom
+                    wgmma_m64k16<256, kBF16>(acc, make_kmajor_desc<BK>(wts + 32u * k), make_kmajor_desc<BK>(box + 32u * k),
+                                             (ks | k) != 0 ? 1u : 0u, 0);
+                wg_commit();
+                wg_wait<1>();
+                if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+                prev = stage;
+                if (++stage == kStages) { stage = 0; phase ^= 1u; }
+            }
+            wg_wait<0>();
+            wg_fence_regs<128>(acc);
+            if (lane == 0) mbar_arrive(empty_bar(prev));
+
+            int nt, x0, y0, n0;
+            tile_origin(tile, &nt, &x0, &y0, &n0);
+            // fp16: which of this thread's pixels 8j + 2(lane%4) + {0,1} are real output pixels (bit 2j + e); GEMM columns
+            // past the box or outside the image are computed from stale or zero-filled rows and never stored
+            uint64_t live = ~0ull;
+            if constexpr (!kBF16) {
+                const int xr = p.ep.Wout - x0, yr = p.ep.Hout - y0, nr = p.ep.N - n0;
+                if (rows_valid < kCmPixels || xr < p.bw || yr < p.bh || nr < p.bn) {
+                    live = 0;
+#pragma unroll 1
+                    for (int b = 0; b < 64; ++b) {
+                        const int px = 8 * (b >> 1) + 2 * (lane & 3) + (b & 1);
+                        const int xx = px % p.bw, yy = (px / p.bw) % p.bh, nn = px / (p.bw * p.bh);
+                        if (px < rows_valid && xx < xr && yy < yr && nn < nr) live |= 1ull << b;
+                    }
+                }
+            }
+            if (has_res) {
+                mbar_wait(res_bar(g), rphase);
+                rphase ^= 1u;
+            }
+            const float* const sc = p.ep.scale + nt * BN + ch;
+            const float* const sh = p.ep.shift + nt * BN + ch;
+            chmajor_epilogue<kBF16>(
+                acc, __ldg(sc), __ldg(sh), __ldg(sc + 8), __ldg(sh + 8), p.ep.act, has_res ? stg : 0u, 8, [] {},
+                [&](int j) {
+                    return (static_cast<uint32_t>(live >> (2 * j)) & 1u) << 15 | (static_cast<uint32_t>(live >> (2 * j + 1)) & 1u) << 31;
+                },
+                stg, bar_id, leader, &p.tmO, nt * BN + 64 * g, x0, y0, n0);
+            if (has_res && leader && tile + static_cast<int>(gridDim.x) < total_tiles) {
+                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the store has read the staging box
+                fetch_res(tile + gridDim.x);  // lands while both warpgroups run the next tile's MMAs
+            }
+        }
+        if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
     } else {
         setmaxnreg_inc<kConsumerRegs>();
         // =============================== consumer warpgroups: MMA + epilogue ===============================

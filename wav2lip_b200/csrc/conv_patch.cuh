@@ -159,10 +159,6 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
         const uint32_t stg = stg_base + grp * kStgBytes;
         const bool leader = (q == 0 && lane == 0);
         const uint32_t bar_id = 1 + grp;
-        // ldmatrix / stmatrix .x4: lanes 8m .. 8m+7 address the 8 pixel rows of matrix m = (tile row 2i + m/2, 16-byte
-        // channel chunk 2q + m%2), which land in / come from the fragment registers of (row 2i + m/2, channel ch + 8(m%2))
-        const int lm_row = lane >> 4, lm_px = lane & 7;
-        const uint32_t lm_chunk = 16u * (2 * q + ((lane >> 3) & 1));
         const uint32_t sbo_b = static_cast<uint32_t>(p.PW) * kRowBytes;
         uint32_t tap_off[kPatchMaxTaps];
 #pragma unroll
@@ -196,69 +192,23 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
             wg_fence_regs<128>(acc);
             if (p.res_row < 0 && lane == 0) mbar_arrive(empty_bar(stage));  // the MMAs were the patch's last readers
 
-            // folded BatchNorm, then the residual = this block's input = centre of the patch (pixel-major, swizzled by
-            // address bits as TMA wrote it), read transposed into the fragment layout
-            const uint32_t res_base = a_base + stage * kc * p.patch_stride;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    float* a = acc + 8 * i + 4 * h;
-                    a[0] = fmaf(a[0], sc0, sh0); a[1] = fmaf(a[1], sc0, sh0);
-                    a[2] = fmaf(a[2], sc1, sh1); a[3] = fmaf(a[3], sc1, sh1);
-                }
-                if (p.res_row >= 0) {
-                    uint32_t ad = res_base + static_cast<uint32_t>(p.res_row + (2 * i + lm_row) * p.PW + lm_px) * kRowBytes + lm_chunk;
-                    ad ^= ((ad >> 7) & 7u) << 4;
-                    uint32_t rv[4];
-                    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-                                 : "=r"(rv[0]), "=r"(rv[1]), "=r"(rv[2]), "=r"(rv[3]) : "r"(ad));
-#pragma unroll
-                    for (int m = 0; m < 4; ++m) {
-                        const float2 v = unpack2<kBF16>(rv[m]);
-                        acc[8 * i + 2 * m] += v.x;
-                        acc[8 * i + 2 * m + 1] += v.y;
-                    }
-                }
-            }
-            if (p.res_row >= 0) {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty_bar(stage));  // this warp is done with the patch
-            }
-            if (e.act == ACT_RELU) {
-#pragma unroll
-                for (int j = 0; j < 128; ++j) acc[j] = fmaxf(acc[j], 0.0f);
-            } else if (e.act == ACT_LRELU) {
-#pragma unroll
-                for (int j = 0; j < 128; ++j) acc[j] = acc[j] > 0.0f ? acc[j] : 0.01f * acc[j];
-            }
-            // stage the tile (pixel-major rows of 64 channels, 128-byte swizzle) by stmatrix.trans and TMA-store it; only
-            // pixels inside the image may raise the fp16 range flag
+            // folded BatchNorm, the residual = this block's input = centre of the patch (pixel-major, swizzled by address
+            // bits as TMA wrote it, output rows PW pixels apart), the activation, then the 8 x 32 tile leaves by one TMA
+            // store.  Column chunk j of the fragment is tile row j: only pixels inside the image may raise the fp16 flag.
             const int x = tx * kPatchTileW + px;
             const uint32_t live_x = (x < e.Wout ? 0x8000u : 0u) | (x + 1 < e.Wout ? 0x80000000u : 0u);
             const int rows_live = e.Hout - ty * kTileH;
-            if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the buffer
-            named_bar_sync(bar_id, 128);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                uint32_t ad = stg + static_cast<uint32_t>((2 * i + lm_row) * kPatchTileW + lm_px) * kRowBytes + lm_chunk;
-                ad ^= ((ad >> 7) & 7u) << 4;
-                const uint32_t l0 = 2 * i < rows_live ? live_x : 0u, l1 = 2 * i + 1 < rows_live ? live_x : 0u;
-                const uint32_t o0 = pack2_live<kBF16>(acc[8 * i + 0], acc[8 * i + 1], l0);
-                const uint32_t o1 = pack2_live<kBF16>(acc[8 * i + 2], acc[8 * i + 3], l0);
-                const uint32_t o2 = pack2_live<kBF16>(acc[8 * i + 4], acc[8 * i + 5], l1);
-                const uint32_t o3 = pack2_live<kBF16>(acc[8 * i + 6], acc[8 * i + 7], l1);
-                asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1,%2,%3,%4};"
-                             ::"r"(ad), "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
-            named_bar_sync(bar_id, 128);
-            if (leader) {
-                asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                             ::"l"(reinterpret_cast<uint64_t>(&p.tmO)), "r"(stg), "r"(0), "r"(tx * kPatchTileW), "r"(ty * kTileH), "r"(n)
-                             : "memory");
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
+            const uint32_t res = p.res_row >= 0 ? a_base + (stage * kc * p.patch_stride + p.res_row * kRowBytes) : 0u;
+            chmajor_epilogue<kBF16>(
+                acc, sc0, sh0, sc1, sh1, e.act, res, p.PW,
+                [&] {
+                    if (p.res_row >= 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(empty_bar(stage));  // this warp is done with the patch
+                    }
+                },
+                [&](int j) { return j < rows_live ? live_x : 0u; }, stg, bar_id, leader, &p.tmO, 0, tx * kPatchTileW,
+                ty * kTileH, n);
         }
         if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
     } else {

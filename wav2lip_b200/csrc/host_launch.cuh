@@ -7,14 +7,18 @@
 // conv kernel dispatch
 // ------------------------------------------------------------------------------------------------
 typedef void (*ConvKernelFn)(const ConvParams);
-struct ConvKernelEntry { int BN, BK; bool bf16, head; ConvKernelFn fn; int smem; uint64_t attr_set; int mt; int threads; };
+// cm: the channel-major form of the (BN, BK, MT = 1) instantiation (conv_igemm.cuh, kCM)
+struct ConvKernelEntry { int BN, BK; bool bf16, head; ConvKernelFn fn; int smem; uint64_t attr_set; int mt; int threads; bool cm; };
 
 #define W2L_CONV_ENTRY(BN_, BK_)                                                                                                        \
-    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads}, \
-    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads}
+    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads, false}, \
+    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false>, ConvCfg<BN_, BK_>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_>::kThreads, false}
 #define W2L_CONV_ENTRY_MT2(BN_, BK_)                                                                                                    \
-    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads}, \
-    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads}
+    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads, false}, \
+    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false, 2>, ConvCfg<BN_, BK_, 2>::kSmemBytes, 0, 2, ConvCfg<BN_, BK_, 2>::kThreads, false}
+#define W2L_CONV_ENTRY_CM(BN_, BK_)                                                                                                     \
+    {BN_, BK_, false, false, conv_igemm_kernel<BN_, BK_, false, false, 1, true>, ConvCfg<BN_, BK_, 1, true>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_, 1, true>::kThreads, true}, \
+    {BN_, BK_, true, false, conv_igemm_kernel<BN_, BK_, true, false, 1, true>, ConvCfg<BN_, BK_, 1, true>::kSmemBytes, 0, 1, ConvCfg<BN_, BK_, 1, true>::kThreads, true}
 
 static ConvKernelEntry g_conv_kernels[] = {
     W2L_CONV_ENTRY(16, 16), W2L_CONV_ENTRY(16, 32), W2L_CONV_ENTRY(16, 64),
@@ -22,13 +26,14 @@ static ConvKernelEntry g_conv_kernels[] = {
     W2L_CONV_ENTRY(64, 16), W2L_CONV_ENTRY(64, 32), W2L_CONV_ENTRY(64, 64),
     W2L_CONV_ENTRY(128, 16), W2L_CONV_ENTRY(128, 32), W2L_CONV_ENTRY(128, 64),
     W2L_CONV_ENTRY_MT2(64, 64), W2L_CONV_ENTRY_MT2(64, 32),
-    {32, 16, false, true, conv_igemm_kernel<32, 16, false, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads},
-    {32, 16, true, true, conv_igemm_kernel<32, 16, true, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads},
+    W2L_CONV_ENTRY_CM(128, 64),
+    {32, 16, false, true, conv_igemm_kernel<32, 16, false, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads, false},
+    {32, 16, true, true, conv_igemm_kernel<32, 16, true, true>, ConvCfg<32, 16>::kSmemBytes, 0, 1, ConvCfg<32, 16>::kThreads, false},
 };
 
-static ConvKernelEntry* find_conv_kernel(int BN, int BK, bool bf16, bool head, int mt = 1) {
+static ConvKernelEntry* find_conv_kernel(int BN, int BK, bool bf16, bool head, int mt = 1, bool cm = false) {
     for (auto& e : g_conv_kernels)
-        if (e.BN == BN && e.BK == BK && e.bf16 == bf16 && e.head == head && e.mt == mt) return &e;
+        if (e.BN == BN && e.BK == BK && e.bf16 == bf16 && e.head == head && e.mt == mt && e.cm == cm) return &e;
     return nullptr;
 }
 
@@ -116,8 +121,8 @@ static int launch_conv(w2l_ctx* ctx, const Op& op, cudaStream_t st, bool pdl = t
         ctx->launches++;
         return W2L_OK;
     }
-    ConvKernelEntry* e = find_conv_kernel(op.BN, op.BK, ctx->bf16, op.head, op.MT);
-    if (!e) return fail(W2L_EINVAL, "no conv kernel for BN=%d BK=%d head=%d MT=%d", op.BN, op.BK, (int)op.head, op.MT);
+    ConvKernelEntry* e = find_conv_kernel(op.BN, op.BK, ctx->bf16, op.head, op.MT, op.cm);
+    if (!e) return fail(W2L_EINVAL, "no conv kernel for BN=%d BK=%d head=%d MT=%d cm=%d", op.BN, op.BK, (int)op.head, op.MT, (int)op.cm);
     CKR(ensure_smem_attr(&e->attr_set, ctx->device, (const void*)e->fn, e->smem));
     CK(launch_k(e->fn, op.grid, e->threads, (size_t)e->smem, st, op.cp, pdl));
     ctx->launches++;

@@ -8,16 +8,23 @@
 // ------------------------------------------------------------------------------------------------
 static int pick_bk(int cin_pad) { return (cin_pad % 64 == 0) ? 64 : (cin_pad % 32 == 0) ? 32 : 16; }
 static int round_up(int a, int b) { return (a + b - 1) / b * b; }
+// channel-major selection (make_conv_op), set from the per-launch times of the generator at N = 640 on an H100 SXM (DESIGN
+// section 6): least K steps per tile, least K steps per CTA (rounds x K steps: the pipeline fill and the exposed epilogues are
+// amortised over it), and how much worse than the row-major tiles' the fill of the grid's rounds may be
+constexpr int kCmMinSteps = 18;
+constexpr int kCmMinCtaSteps = 48;
+constexpr double kCmFillMargin = 0.06;
 
-// The 128-row tile is a (bw x bh x bn) box of output pixels; choose the box with the least padding waste.
-static void pick_box(int W, int H, int N, int sx, int sy, int* bw, int* bh, int* bn) {
+// A tile of `pixels` GEMM rows (columns in the channel-major form) is a (bw x bh x bn) box of output pixels; choose the
+// box with the least padding waste.
+static void pick_box(int W, int H, int N, int sx, int sy, int* bw, int* bh, int* bn, int pixels = kTileM) {
     double best = 1e30;
     int b_w = 1, b_h = 1, b_n = 1;
-    for (int w = 1; w <= std::min(W, kTileM); ++w) {
+    for (int w = 1; w <= std::min(W, pixels); ++w) {
         if (w * sx > 256) break;
-        for (int h = 1; h <= std::min(H, kTileM / w); ++h) {
+        for (int h = 1; h <= std::min(H, pixels / w); ++h) {
             if (h * sy > 256) break;
-            int n = std::min(kTileM / (w * h), std::max(N, 1));
+            int n = std::min(pixels / (w * h), std::max(N, 1));
             if (n < 1) continue;
             if (n > 256) n = 256;
             const double tiles = (double)((W + w - 1) / w) * ((H + h - 1) / h) * ((N + n - 1) / n);
@@ -232,19 +239,45 @@ static int make_conv_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a) {
     const int BK = pick_bk(w.cin_pad);
     int bw, bh, bn;
     pick_box(a.Wl, a.Hl, a.in.N, a.sx, a.sy, &bw, &bh, &bn);
-    const int tiles_x = (a.Wl + bw - 1) / bw, tiles_y = (a.Hl + bh - 1) / bh, tiles_n = (a.in.N + bn - 1) / bn;
-    const int m_tiles = tiles_x * tiles_y * tiles_n;
+    int tiles_x = (a.Wl + bw - 1) / bw, tiles_y = (a.Hl + bh - 1) / bh, tiles_n = (a.in.N + bn - 1) / bn;
+    int m_tiles = tiles_x * tiles_y * tiles_n;
     int BN = 16;
     for (int cand : {128, 64, 32, 16})
         if (a.cout % cand == 0) { BN = cand; break; }
     if (a.head) BN = 32;
     else
         while (BN > 32 && m_tiles * (a.cout / BN) < ctx->num_sms && a.cout % (BN / 2) == 0) BN /= 2;
+    // Channel-major form (conv_igemm.cuh, kCM): 128 output channels x a box of kCmPixels pixels per tile, both consumer
+    // warpgroups on every tile, so no epilogue hides behind the other warpgroup's MMAs.  Taken for 16-bit staged outputs
+    // with unit pixel strides (the interleaved phase stores of transposed convs did not gain) when a tile has at least
+    // kCmMinSteps K steps and a CTA at least kCmMinCtaSteps, and the tiles fill the persistent grid's rounds nearly as
+    // well as 128 x 128 row-major tiles: fill = useful pixels x channels over rounds x SMs x tile size.
+    const int k_steps = w.ntaps * (w.cin_pad / BK);
+    if (ctx->use_tma_epi && !ctx->x2 && !a.head && !a.out.f32 && a.cout % 128 == 0 && w.cout_pad % 128 == 0 && BK == 64 &&
+        a.osx == 1 && a.osy == 1 && k_steps >= kCmMinSteps) {
+        int cw, ch, cn;
+        pick_box(a.Wl, a.Hl, a.in.N, a.sx, a.sy, &cw, &ch, &cn, kCmPixels);
+        const long long cm_tiles = (long long)((a.Wl + cw - 1) / cw) * ((a.Hl + ch - 1) / ch) * ((a.in.N + cn - 1) / cn);
+        const int S = ctx->num_sms, nt = a.cout / 128;
+        auto fill = [&](long long tiles, int pixels) {
+            const long long rounds = (tiles * nt + S - 1) / S;
+            return (double)a.Wl * a.Hl * a.in.N / ((double)rounds * S * pixels / nt);
+        };
+        if ((cm_tiles * nt + S - 1) / S * k_steps >= kCmMinCtaSteps &&
+            fill(cm_tiles, kCmPixels) >= (1.0 - kCmFillMargin) * fill(m_tiles, kTileM)) {
+            op.cm = true;
+            op.name += " [cm]";
+            BN = 128;
+            bw = cw; bh = ch; bn = cn;
+            tiles_x = (a.Wl + bw - 1) / bw; tiles_y = (a.Hl + bh - 1) / bh; tiles_n = (a.in.N + bn - 1) / bn;
+            m_tiles = tiles_x * tiles_y * tiles_n;
+        }
+    }
     if (w.cout_pad % BN != 0) return fail(W2L_EINVAL, "%s: cout_pad %d vs BN %d", a.name.c_str(), w.cout_pad, BN);
     op.BN = BN; op.BK = BK; op.head = a.head;
     // two M tiles per CTA (shared weight slab, one consumer warpgroup each) once there is plenty of work
     const int n_tiles_ = a.cout / BN;
-    if (ctx->use_mt2 && !a.head && find_conv_kernel(BN, BK, ctx->bf16, false, 2) &&
+    if (ctx->use_mt2 && !a.head && !op.cm && find_conv_kernel(BN, BK, ctx->bf16, false, 2) &&
         (long long)((m_tiles + 1) / 2) * n_tiles_ >= 2LL * ctx->num_sms)
         op.MT = 2;
     if (op.MT == 2) op.name += " [2M]";

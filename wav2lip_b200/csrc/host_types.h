@@ -183,6 +183,7 @@ struct Op {
     // conv
     ConvParams cp;
     int BN = 0, BK = 0, MT = 1;
+    bool cm = false;     // channel-major form of the generic kernel (BN channels on wgmma's M, kCmPixels pixels on N)
     bool head = false;
     int grid = 0;
     double flops = 0;  // algorithmic (true MACs*2), not padded

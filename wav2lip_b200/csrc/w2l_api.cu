@@ -660,7 +660,16 @@ int w2l_debug_kernel_table(int cap, w2l_kernel_info* out) {
         k.family = fam; k.bn = bn; k.bk = bk; k.mt = mt; k.head = head ? 1 : 0; k.bf16 = bf16 ? 1 : 0;
         t.push_back(k);
     };
-    for (const auto& e : g_conv_kernels) add(W2L_KFAM_IGEMM, e.BN, e.BK, e.mt, e.head, e.bf16);
+    // one row per (family, BN, BK, MT, head, precision); an instantiation that also has the channel-major form is
+    // named "[cm]"
+    for (const auto& e : g_conv_kernels)
+        if (!e.cm) add(W2L_KFAM_IGEMM, e.BN, e.BK, e.mt, e.head, e.bf16);
+    for (const auto& e : g_conv_kernels)
+        if (e.cm)
+            for (auto& k : t)
+                if (k.family == W2L_KFAM_IGEMM && k.bn == e.BN && k.bk == e.BK && k.mt == e.mt && k.head == (e.head ? 1 : 0) &&
+                    k.bf16 == (e.bf16 ? 1 : 0))
+                    snprintf(k.name, sizeof(k.name), "[cm]");
     for (const auto& e : g_patch_kernels) add(W2L_KFAM_PATCH, e.BN, e.BK, 1, e.head, e.bf16);
     for (const auto& e : g_ct_kernels) add(W2L_KFAM_CONVT_FUSED, kCtBN, e.BK, 1, false, e.bf16);
     if (!out) return (int)t.size();
