@@ -244,6 +244,79 @@ int64_t w2l_mel_num_chunks(int64_t n_frames, double fps);
 int w2l_mel_chunks(w2l_ctx* ctx, const float* mel_dev, int64_t n_frames, double fps, float* chunks_dev,
                    int64_t n_chunks, void* stream);
 
+/* ---- streaming ---- */
+/* Streaming form of w2l_melspectrogram: audio arrives in pieces, frames come out as soon as they are final, and every
+ * frame is bit-identical to the same column of w2l_melspectrogram on the whole utterance.  Frame f is final once
+ * 200 f + 400 <= L (L = samples received); the frames that reach the end of the utterance need its length and come out
+ * of _finish.  Audio and mel live in device rings of fixed size (audio_ring_log2: log2 of the audio ring in samples,
+ * 11..24, 0 = 16; the mel ring follows from it); a push of any length is split internally, so device memory does not
+ * grow with the stream.
+ *   pcm: fp32 16 kHz samples in host memory (pageable or pinned) or in device memory of the context's device.
+ *   _push writes the newly final frames to mel_dev as an (80, n_new) row-major block; *n_new may be 0.  The caller
+ *   sizes mel_dev with w2l_melstream_pending (frames a push of n_samples more, or the finish, will write).
+ *   _finish writes the remaining frames; the stream then has 1 + L/200 frames in all (L >= 2).
+ *   *nan_seen (optional, synchronises the stream) reports whether any frame so far held a NaN (the reference raises
+ *   on that, inference.py:228-229).
+ * Calls are asynchronous on `stream` except where stated.  pcm may be reused when _push returns if it is host memory
+ * (for pinned memory _push waits for its copies, and so for the work queued on `stream` before them); device pcm is
+ * read by work queued on `stream`, ordered like any other asynchronous copy there. */
+typedef struct w2l_melstream w2l_melstream;
+int w2l_melstream_create(w2l_ctx* ctx, int audio_ring_log2, w2l_melstream** out);
+int64_t w2l_melstream_pending(const w2l_melstream* ms, int64_t n_samples, int finish);
+int w2l_melstream_push(w2l_melstream* ms, const float* pcm, int64_t n_samples, float* mel_dev, int64_t cap_frames,
+                       int64_t* n_new, int* nan_seen, void* stream);
+int w2l_melstream_finish(w2l_melstream* ms, float* mel_dev, int64_t cap_frames, int64_t* n_new, int* nan_seen,
+                         void* stream);
+int w2l_melstream_destroy(w2l_melstream* ms);
+
+/* Streaming lip-sync session: the whole inference loop of inference.py (:224-244 mel and chunks, :87-103 boxes,
+ * :120-140 and :259-271 generator and paste) on audio that arrives in pieces, for a fixed face video.  Each output
+ * frame is emitted as soon as the audio received so far fixes it, and the concatenated output equals the offline loop
+ * bit for bit.  Output i shows frame i % n_total (n_total = min(chunk count, F), inference.py:244) with mel chunk i.
+ *
+ * The video and its boxes: frames_dev (F,H,W,3) uint8 on the device (it must stay valid while the session lives), and
+ * either F detector rects (x1,y1,x2,y2 per frame, as get_detections_for_batch returns them) that the session pads,
+ * clips and smooths as inference.py:87-103 does (the smoothing of inference.py:59-66 over the first n_total frames;
+ * d->nosmooth turns it off), or one fixed box (d->has_box, d->box = y1,y2,x1,x2: inference.py:116-119). */
+typedef struct w2l_stream_desc {
+    int32_t F, H, W;     /* video frames and size */
+    double fps;          /* chunk start s_i = int(i * 80./fps), inference.py:232 */
+    int32_t nosmooth;
+    int32_t has_box;     /* 1: box below for every frame; rects unused */
+    int32_t box[4];      /* y1, y2, x1, x2 */
+    int32_t pads[4];     /* top, bottom, left, right (inference.py --pads, default 0 10 0 0) */
+} w2l_stream_desc;
+
+/* One emitted row: output index, mel chunk start (absolute mel frame), video frame index, box y1, y2, x1, x2. */
+#define W2L_STREAM_ROW 7
+
+/* Pure host function (no device, no context): the rows that n_samples received audio samples fix, or, with
+ * final != 0, all rows of an utterance of n_samples.  *n_fixed gets their count; rows [first_row, first_row + cap)
+ * of them (those that exist) are written to rows_host as W2L_STREAM_ROW int32 each.  rects_host: F x 4, unused with a
+ * fixed box.  A final length with fewer than 16 mel frames is W2L_EINVAL (there is no chunk). */
+int w2l_stream_schedule(const w2l_stream_desc* d, const int32_t* rects_host, int64_t n_samples, int final_,
+                        int64_t first_row, int64_t cap, int32_t* rows_host, int64_t* n_fixed);
+
+/* Every step runs the generator at exactly `batch` rows (one plan; rows past the ready ones repeat the last ready row
+ * and are dropped), from a CUDA graph captured once per session and replayed (W2L_DISABLE_STREAMGRAPH=1 launches the
+ * same kernels directly).  The generator weights must be loaded; loading new ones between pushes is allowed.
+ * _push / _finish write n_out output frames (n_out, H, W, 3) uint8 to out_dev; they are output indices
+ * first_index .. first_index + n_out - 1.  Size out_dev with w2l_stream_pending.  A push whose audio gives a mel frame
+ * holding a NaN fails with W2L_EINVAL and the reference's message (inference.py:228-229) and writes no frame of a
+ * chunk that contains it; so does every later call.  The session must be destroyed before its context.
+ * The mel work runs on a stream of the session's own: a push waits on the host for its own new mel frames and their
+ * NaN flag (host pcm is then copied), not for the steps already queued on `stream`; device pcm makes the mel work wait
+ * for the work queued on `stream` first.  Steps, pastes and outputs are ordered on `stream`. */
+typedef struct w2l_stream w2l_stream;
+int w2l_stream_create(w2l_ctx* ctx, const uint8_t* frames_dev, const w2l_stream_desc* d, const int32_t* rects_host,
+                      int batch, w2l_stream** out);
+int w2l_stream_pending(const w2l_stream* s, int64_t n_samples, int finish, int64_t* n_out);
+int w2l_stream_push(w2l_stream* s, const float* pcm, int64_t n_samples, uint8_t* out_dev, int64_t cap,
+                    int64_t* first_index, int64_t* n_out, void* stream);
+int w2l_stream_finish(w2l_stream* s, uint8_t* out_dev, int64_t cap, int64_t* first_index, int64_t* n_out,
+                      void* stream);
+int w2l_stream_destroy(w2l_stream* s);
+
 /* ---- test aids ---- */
 /* keep every block output of subsequent plans addressable (no buffer reuse) for w2l_debug_layer_output */
 int w2l_set_debug(w2l_ctx* ctx, int keep_all_layer_outputs);

@@ -28,6 +28,15 @@ with torch.no_grad():
     cr = g.crop_resize(frames, boxes)
     pa = g.paste(u[:2], frames, boxes)
     fr = g.infer_frames(torch.rand(2, 1, 80, 16).cuda(), frames, boxes)
+    # streaming: the ring mel kernel (host and device pieces, a wrapping 2^11 ring, the end reflection), the chunk
+    # gather, and a session step uncaptured and replayed from its graph
+    msr = audio.MelStream(0, 11)
+    mw = np.random.randn(7000).astype(np.float32)
+    mparts = [msr.push(mw[:3000]), msr.push(torch.from_numpy(mw[3000:6100]).cuda()).cpu().numpy(), msr.finish()]
+    from wav2lip_b200.stream import LipSyncSession
+    sess = LipSyncSession(g, frames, 25.0, rects=[(7, 5, 80, 60), (0, 0, 88, 62)], batch=2)
+    sfr = [sess.push(np.random.randn(3200).astype(np.float32))[1] for _ in range(3)] + [sess.finish()[1]]
+    sess.close()
     # many units of 128-channel tiles: a 128-channel residual block and a transposed-conv phase set
     from wav2lip_b200.models.conv import Conv2d, Conv2dTranspose
     sw = Conv2d(128, 128, 3, 1, 1, residual=True).cuda().eval()(torch.rand(140, 128, 24, 24).cuda())

@@ -35,7 +35,11 @@ EXPORTS = [
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
     "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
     "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
+    "w2l_melstream_create", "w2l_melstream_pending", "w2l_melstream_push", "w2l_melstream_finish", "w2l_melstream_destroy",
+    "w2l_stream_schedule", "w2l_stream_create", "w2l_stream_pending", "w2l_stream_push", "w2l_stream_finish",
+    "w2l_stream_destroy",
 ]
+STREAM_ROW = 7  # W2L_STREAM_ROW: output index, chunk start, frame index, y1, y2, x1, x2
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
 WG_PLAIN, WG_STRIDED, WG_TRANSPOSED, WG_SWAP, WG_FOLDED = 0, 1, 2, 3, 4
 TAPE_X, TAPE_Z, TAPE_Y, TAPE_DY, TAPE_DZ, TAPE_DU, TAPE_DX, TAPE_DX_ADD, TAPE_STATS = range(9)
@@ -43,6 +47,12 @@ TAPE_X, TAPE_Z, TAPE_Y, TAPE_DY, TAPE_DZ, TAPE_DU, TAPE_DX, TAPE_DX_ADD, TAPE_ST
 
 class W2LError(RuntimeError):
     pass
+
+
+class StreamDesc(C.Structure):
+    """w2l_stream_desc (include/w2l.h)."""
+    _fields_ = [("F", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("fps", C.c_double), ("nosmooth", C.c_int32),
+                ("has_box", C.c_int32), ("box", C.c_int32 * 4), ("pads", C.c_int32 * 4)]
 
 
 class LayerInfo(C.Structure):
@@ -180,6 +190,19 @@ def get_lib() -> C.CDLL:
     lib.w2l_debug_train_blocks.argtypes = [vp, i32, i32, C.POINTER(TrainBlockInfo)]
     lib.w2l_debug_train_tensor.argtypes = [vp, i32, i32, i32, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
                                            C.POINTER(i32), vp]
+    pi64 = C.POINTER(i64)
+    lib.w2l_melstream_create.argtypes = [vp, i32, C.POINTER(vp)]
+    lib.w2l_melstream_pending.argtypes = [vp, i64, i32]
+    lib.w2l_melstream_pending.restype = i64
+    lib.w2l_melstream_push.argtypes = [vp, vp, i64, vp, i64, pi64, C.POINTER(i32), vp]
+    lib.w2l_melstream_finish.argtypes = [vp, vp, i64, pi64, C.POINTER(i32), vp]
+    lib.w2l_melstream_destroy.argtypes = [vp]
+    lib.w2l_stream_schedule.argtypes = [C.POINTER(StreamDesc), vp, i64, i32, i64, i64, vp, pi64]
+    lib.w2l_stream_create.argtypes = [vp, vp, C.POINTER(StreamDesc), vp, i32, C.POINTER(vp)]
+    lib.w2l_stream_pending.argtypes = [vp, i64, i32, pi64]
+    lib.w2l_stream_push.argtypes = [vp, vp, i64, vp, i64, pi64, pi64, vp]
+    lib.w2l_stream_finish.argtypes = [vp, vp, i64, pi64, pi64, vp]
+    lib.w2l_stream_destroy.argtypes = [vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here == header / library mismatch
     if lib.w2l_abi_version() != 1:

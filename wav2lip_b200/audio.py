@@ -140,3 +140,87 @@ def mel_basis() -> np.ndarray:
     out = np.empty((80, 401), dtype=np.float32)
     L.check(L.get_lib().w2l_mel_basis_host(out.ctypes.data_as(C.c_void_p)))
     return out
+
+
+class MelStream:
+    """Streaming `melspectrogram`: push 16 kHz float32 audio as it arrives and get back the mel frames it makes final
+    (frame f once 200 f + 400 samples have arrived), each bit-identical to the same column of `melspectrogram` on the
+    whole utterance; `finish()` returns the frames that reach the end (1 + L // 200 frames in all).  Device memory is
+    two fixed rings (`ring_log2`: log2 of the audio ring in samples, 11..24, default 16), whatever the stream's length.
+
+    `push(pcm)` takes a 1-D numpy array / CPU tensor (returns an (80, k) numpy array) or a CUDA tensor on this stream's
+    device (returns an (80, k) CUDA tensor, on the current stream).  `nan_seen()` reports whether any frame so far held
+    a NaN (inference.py raises on that)."""
+
+    def __init__(self, device: int = 0, ring_log2: int = 0):
+        import torch
+        self._torch = torch
+        self._ctx = _context(int(device))
+        self._lib = self._ctx.lib
+        h = C.c_void_p()
+        _lib().check(self._lib.w2l_melstream_create(self._ctx.h, int(ring_log2), C.byref(h)))
+        self._h = h
+        self.device = int(device)
+        self._cuda_out = False   # finish() answers in the kind of the pushes
+        self._nan_at_finish = None
+
+    def _run(self, pcm, finish: bool):
+        torch = self._torch
+        L = _lib()
+        dev = torch.device("cuda", self.device)
+        on_device = isinstance(pcm, torch.Tensor) and pcm.is_cuda
+        keep = None
+        if pcm is None:
+            ptr, n = None, 0
+            on_device = self._cuda_out
+        elif on_device:
+            if pcm.device != dev:
+                raise ValueError(f"pcm is on {pcm.device}, the stream on {dev}")
+            keep = pcm.detach().reshape(-1).contiguous().float()
+            ptr, n = C.c_void_p(keep.data_ptr()), keep.numel()
+            self._cuda_out = True
+        else:
+            x = pcm.detach().cpu().numpy() if isinstance(pcm, torch.Tensor) else pcm
+            keep = np.ascontiguousarray(np.asarray(x, dtype=np.float32).reshape(-1))
+            ptr, n = keep.ctypes.data_as(C.c_void_p), keep.shape[0]
+        k = int(self._lib.w2l_melstream_pending(self._h, n, 1 if finish else 0))
+        out = torch.empty((80, k), device=dev, dtype=torch.float32)
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        got = C.c_int64()
+        optr = C.c_void_p(out.data_ptr()) if k else None
+        if finish:
+            flag = C.c_int(0)
+            L.check(self._lib.w2l_melstream_finish(self._h, optr, k, C.byref(got), C.byref(flag), stream))
+            self._nan_at_finish = bool(flag.value)
+        else:
+            L.check(self._lib.w2l_melstream_push(self._h, ptr, n, optr, k, C.byref(got), None, stream))
+        assert got.value == k
+        return out if on_device else out.cpu().numpy()
+
+    def push(self, pcm):
+        return self._run(pcm, False)
+
+    def finish(self):
+        """The last frames; call once, after the last push.  A CUDA tensor if any push was a CUDA tensor, else numpy."""
+        return self._run(None, True)
+
+    def nan_seen(self) -> bool:
+        """Whether any frame so far held a NaN (synchronises the current stream)."""
+        if self._nan_at_finish is not None:
+            return self._nan_at_finish
+        torch = self._torch
+        flag, got = C.c_int(0), C.c_int64()
+        stream = C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream)
+        _lib().check(self._lib.w2l_melstream_push(self._h, None, 0, None, 0, C.byref(got), C.byref(flag), stream))
+        return bool(flag.value)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.w2l_melstream_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -63,5 +63,6 @@ static int init_mel_tables(w2l_ctx* ctx) {
     CK(cudaMemcpy(ctx->mel_bstart, start.data(), MEL_BANDS * 4, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->mel_blen, len.data(), MEL_BANDS * 4, cudaMemcpyHostToDevice));
     CK(cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMelSmemBytes));
+    CK(cudaFuncSetAttribute(mel_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMelSmemBytes));
     return W2L_OK;
 }

@@ -375,16 +375,17 @@ static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, 
     auto it = ctx->plans.find(key);
     if (it != ctx->plans.end()) { it->second->last_used = ++ctx->plan_clock; *out = it->second.get(); return W2L_OK; }
     if (!ctx->nets[net].loaded) return fail(W2L_ESTATE, "weights of net %d not loaded", net);
-    // keep at most a few plans per net alive (activation arenas are large): evict the least recently used
+    // keep at most a few plans per net alive (activation arenas are large): evict the least recently used one that no
+    // streaming session has pinned (a pinned plan is baked into that session's CUDA graph)
     for (;;) {
         int count = 0;
         auto lru = ctx->plans.end();
         for (auto p = ctx->plans.begin(); p != ctx->plans.end(); ++p)
             if (p->second->net == net) {
                 ++count;
-                if (lru == ctx->plans.end() || p->second->last_used < lru->second->last_used) lru = p;
+                if (p->second->pins == 0 && (lru == ctx->plans.end() || p->second->last_used < lru->second->last_used)) lru = p;
             }
-        if (count < 6) break;
+        if (count < 6 || lru == ctx->plans.end()) break;
         CK(cudaDeviceSynchronize());  // the plan's buffers may still be in use by queued launches
         if (ctx->last_plan[net] == lru->second.get()) ctx->last_plan[net] = nullptr;
         ctx->plans.erase(lru);

@@ -224,6 +224,7 @@ struct Plan {
     std::vector<DevMem<>> allocs;
     std::map<int, Act> layer_out;  // layer index -> activation view (debug export)
     long long last_used = 0;       // LRU stamp
+    int pins = 0;                  // streaming sessions replaying it from a CUDA graph: exempt from LRU eviction
     bool x2 = false;               // split-operand precision: activations carry hi and lo planes
     bool has_side = false;         // some ops run on the side stream
     std::unique_ptr<S3fdDetWork> det;  // S3FD: detection workspace (nullptr until the first w2l_s3fd_detect_u8)
@@ -251,10 +252,14 @@ struct w2l_ctx {
     bool use_ctfused = true;  // W2L_DISABLE_CTFUSED=1
     bool use_fold = true;   // W2L_DISABLE_FOLD=1 / driver rejects overlapping-stride tensor maps
     bool use_pdl = true;      // W2L_DISABLE_PDL=1
+    bool use_stream_graph = true;  // W2L_DISABLE_STREAMGRAPH=1: streaming-session steps launched one by one, not replayed
     NetW nets[4];
     DevMem<float> s3fd_l2w[3];   // conv3_3_norm / conv4_3_norm / conv5_3_norm weights (fp32 copies)
     std::map<std::string, std::unique_ptr<Plan>> plans;
     Plan* last_plan[4] = {nullptr, nullptr, nullptr, nullptr};
+    // bumped whenever drop_plans erases the plans of a net (new weights): a streaming session whose graph was captured
+    // under an older epoch drops its plan pointer and graph and captures again
+    uint64_t plan_epoch[4] = {0, 0, 0, 0};
     std::vector<w2l_kernel_info> last_block_kernels;  // conv launches of the last w2l_conv_block_forward (its plan is freed)
     int64_t launches = 0;
     long long plan_clock = 0;

@@ -177,4 +177,5 @@ static void drop_plans(w2l_ctx* ctx, int net) {
         else ++it;
     }
     ctx->last_plan[net] = nullptr;
+    ctx->plan_epoch[net]++;
 }

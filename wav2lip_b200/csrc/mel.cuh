@@ -95,7 +95,26 @@ __device__ __forceinline__ double2 shfl_d2(double2 v, int src_lane) {
     return make_double2(__shfl_sync(0xffffffffu, v.x, src_lane, 16), __shfl_sync(0xffffffffu, v.y, src_lane, 16));
 }
 
-__global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) {
+// The load stage and the store stage are template parameters; everything between them (window, FFT, magnitude, mel
+// product, dB, normalise, clip) is shared, so a frame computed by either kernel below has the same bits.
+//   Src::len()     the length the reflection at the end uses
+//   Src::x(j, d)   sample j + d (absolute index, 0 <= j + d < len())
+//   Dst::put(m, t, v)   writes band m of frame t (called with consecutive t across a block's frames)
+//   Dst::note(s)   sees every pre-clip mel sum
+// The block computes frames [f0 + blockIdx.x * MEL_FPB, ...) below f1.
+struct MelWavSrc {      // the whole utterance in device memory (w2l_melspectrogram)
+    const MelParams& p;
+    __device__ __forceinline__ long long len() const { return p.L; }
+    __device__ __forceinline__ double x(long long j, int d) const { return (double)__ldg(p.wav + j + d); }
+};
+struct MelDenseDst {    // (80, F) row-major
+    const MelParams& p;
+    __device__ __forceinline__ void note(float) const {}
+    __device__ __forceinline__ void put(int m, long long t, float v) const { p.mel[(long long)m * p.F + t] = v; }
+};
+
+template <class Src, class Dst>
+__device__ __forceinline__ void mel_frames(const MelParams& p, const Src& src, const Dst& dst, long long f0, long long f1) {
     extern __shared__ uint8_t mel_smem[];
     double2* tw = reinterpret_cast<double2*>(mel_smem);                 // [401] exp(-2 pi i m / 800)  (+3 pad)
     double2* ybuf = tw + 404;                                            // [FPB][16][25]
@@ -108,16 +127,16 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) 
     // ---------------- step 1: thread = (frame f, n1) ----------------
     if (tid < MEL_FPB * 25) {
         const int f = tid / 25, n1 = tid % 25;
-        const long long t = (long long)blockIdx.x * MEL_FPB + f;
-        if (t < p.F) {
+        const long long t = f0 + (long long)blockIdx.x * MEL_FPB + f;
+        if (t < f1) {
             double2 v[16];
             const long long base = t * MEL_HOP - MEL_NFFT / 2 + 2 * n1;
 #pragma unroll
             for (int n2 = 0; n2 < 16; ++n2) {
                 const long long j0 = base + 50 * n2;
                 double y0, y1;
-                if (j0 >= 1 && j0 + 1 < p.L) {   // interior: three consecutive samples
-                    const double xm = (double)__ldg(p.wav + j0 - 1), x0 = (double)__ldg(p.wav + j0), x1 = (double)__ldg(p.wav + j0 + 1);
+                if (j0 >= 1 && j0 + 1 < src.len()) {   // interior: three consecutive samples
+                    const double xm = src.x(j0, -1), x0 = src.x(j0, 0), x1 = src.x(j0, 1);
                     y0 = x0 + (-0.97) * xm;
                     y1 = x1 + (-0.97) * x0;
                 } else {                         // np.pad(mode="reflect") of the PRE-EMPHASISED signal
@@ -125,9 +144,9 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) 
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         long long j = j0 + e;
-                        while (j < 0 || j >= p.L) j = j < 0 ? -j : 2 * (p.L - 1) - j;
-                        const double x0 = (double)__ldg(p.wav + j);
-                        yy[e] = (j > 0) ? x0 + (-0.97) * (double)__ldg(p.wav + j - 1) : x0;
+                        while (j < 0 || j >= src.len()) j = j < 0 ? -j : 2 * (src.len() - 1) - j;
+                        const double x0 = src.x(j, 0);
+                        yy[e] = (j > 0) ? x0 + (-0.97) * src.x(j, -1) : x0;
                     }
                     y0 = yy[0]; y1 = yy[1];
                 }
@@ -170,8 +189,8 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) 
     // ---------------- step 3: thread = (frame f, k2), whole warps so that the shuffles below are convergent ----------------
     if (tid < 96) {
         const int f = tid >> 4, k2 = tid & 15;
-        const long long t = (long long)blockIdx.x * MEL_FPB + f;
-        const bool live = f < MEL_FPB && t < p.F;
+        const long long t = f0 + (long long)blockIdx.x * MEL_FPB + f;
+        const bool live = f < MEL_FPB && t < f1;
         double2 y[25];
 #pragma unroll
         for (int n1 = 0; n1 < 25; ++n1) y[n1] = live ? ybuf[f * 400 + k2 * 25 + n1] : make_double2(0.0, 0.0);
@@ -217,12 +236,13 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) 
     // ---------------- sparse mel product + dB + normalise / clip, fp32 as NumPy does on float32 arrays ----------------
     for (int i = tid; i < MEL_BANDS * MEL_FPB; i += MEL_THREADS) {
         const int f = i / MEL_BANDS, m = i % MEL_BANDS;
-        const long long t = (long long)blockIdx.x * MEL_FPB + f;
-        if (t >= p.F) continue;
+        const long long t = f0 + (long long)blockIdx.x * MEL_FPB + f;
+        if (t >= f1) continue;
         const float* mag = mags + f * 404;
         const int off = p.boff[m], st = p.bstart[m], len = p.blen[m];
         float s = 0.0f;
         for (int j = 0; j < len; ++j) s = fmaf(__ldg(p.bvals + off + j), mag[st + j], s);
+        dst.note(s);
         const float db = 20.0f * log10f(fmaxf(1e-5f, s)) - 20.0f;
         float v = 8.0f * ((db + 100.0f) / 100.0f) - 4.0f;
         v = fminf(fmaxf(v, -4.0f), 4.0f);
@@ -231,9 +251,48 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) 
     __syncthreads();
     for (int i = tid; i < MEL_BANDS * MEL_FPB; i += MEL_THREADS) {
         const int m = i / MEL_FPB, ff = i % MEL_FPB;
-        const long long tt = (long long)blockIdx.x * MEL_FPB + ff;
-        if (tt < p.F) p.mel[(long long)m * p.F + tt] = outs[i];
+        const long long tt = f0 + (long long)blockIdx.x * MEL_FPB + ff;
+        if (tt < f1) dst.put(m, tt, outs[i]);
     }
+}
+
+__global__ void __launch_bounds__(MEL_THREADS, 4) mel_kernel(const MelParams p) {
+    mel_frames(p, MelWavSrc{p}, MelDenseDst{p}, 0, p.F);
+}
+
+// ---- streaming form (w2l_melstream_*): audio and mel live in power-of-two rings indexed by absolute position ----
+// Frame f reads pre-emphasised samples [200 f - 400, 200 f + 400) and x[200 f - 401]: the reflection at the start uses
+// absolute indices, so frames 0 and 1 are exact whatever has arrived.  A frame is final once 200 f + 400 <= L; only the
+// frames that reach the end of the utterance reflect there, and they are computed with L = L_end (finish).  A ring slot
+// is read only while it still holds the sample of that absolute index (the host never lets the writer lap the oldest
+// sample a pending frame reads).
+struct MelRingSrc {
+    const float* ring;
+    long long mask;      // ring length - 1
+    long long L;         // L_end at finish; otherwise larger than any index read, so only the start reflects
+    __device__ __forceinline__ long long len() const { return L; }
+    __device__ __forceinline__ double x(long long j, int d) const { return (double)__ldg(ring + ((j + d) & mask)); }
+};
+struct MelRingDst {     // (80, R) row-major ring of frame columns; NaN anywhere in a frame sets *nan (sticky)
+    float* mel;
+    long long pitch;     // R
+    int* nan;
+    __device__ __forceinline__ void note(float s) const { if (s != s) atomicOr(nan, 1); }
+    __device__ __forceinline__ void put(int m, long long t, float v) const { mel[(long long)m * pitch + (t & (pitch - 1))] = v; }
+};
+
+struct MelRingParams {
+    const float* audio;
+    long long audio_mask;
+    float* mel;
+    long long mel_pitch;
+    long long L;          // see MelRingSrc::L
+    long long f0, f1;     // frames to compute
+    int* nan;
+};
+
+__global__ void __launch_bounds__(MEL_THREADS, 4) mel_ring_kernel(const MelParams p, const MelRingParams r) {
+    mel_frames(p, MelRingSrc{r.audio, r.audio_mask, r.L}, MelRingDst{r.mel, r.mel_pitch, r.nan}, r.f0, r.f1);
 }
 
 }  // namespace w2l

@@ -28,6 +28,7 @@
 #include "netspec.h"
 #include "resize.cuh"
 #include "s3fd_detect.cuh"
+#include "stream.cuh"
 #include "train_data.cuh"
 #include "train_kernels.cuh"
 #include "wgrad.cuh"
@@ -41,6 +42,7 @@ using namespace w2l;
 #include "host_plans.cuh"
 #include "host_mel_tables.h"
 #include "host_train.cuh"
+#include "host_stream.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // C-ABI
@@ -111,6 +113,7 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
         ctx->use_ctfused = enabled("W2L_DISABLE_CTFUSED");
         ctx->use_side = enabled("W2L_DISABLE_SIDESTREAM");
         ctx->use_pdl = enabled("W2L_DISABLE_PDL");
+        ctx->use_stream_graph = enabled("W2L_DISABLE_STREAMGRAPH");
         if (ctx->x2) {  // the split-operand mode runs on the generic kernel with the direct epilogue only
             ctx->use_patch = ctx->use_fold = ctx->use_fold_s2 = ctx->use_ctfused = ctx->use_tma_epi = false;
         }
