@@ -22,11 +22,14 @@
 //
 // Two consumer warpgroups take alternate tiles; each issues the wgmma chain of its tile into registers and runs
 // the epilogue, so one group's epilogue overlaps the other's MMAs.  The ring has an even number of stages, so a
-// stage is always consumed by the same warpgroup and its parity waits are in order.  In the epilogue
+// stage is always consumed by the same warpgroup and its parity waits are in order.  The epilogue works on the
+// accumulator fragment itself (no shared-memory transpose):
 //   * the residual of a residual block is the block's own input, i.e. the centre of the patch that is already
-//     in shared memory: it is read from there (the warpgroup releases the patch after that read);
-//   * results are staged in swizzled shared memory and written with ONE TMA tensor store per tile (which also
-//     clips ragged edges), instead of 128 threads x 8 scattered 16-byte stores;
+//     in shared memory: each thread reads its channel pairs from there (the warpgroup releases the patch after that read);
+//   * results are staged as packed 16-bit pairs at the fragment's (pixel, channel pair) in swizzled shared memory and
+//     written with ONE TMA tensor store per tile (which also clips ragged edges);
+//   * the fused 32 -> 3 head gathers each pixel's 32 channels into one lane of its quad (two shuffle steps) and runs
+//     the dot products there in channel order;
 //   * scale/shift/head weights come from the constant bank (kernel params).
 //
 // Channel-major form (BN = 64, BK = 64, no head: the 64 -> 64 residual blocks).  With pixels on M and 64 channels on N,
@@ -78,7 +81,6 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     pdl_launch_dependents();
     constexpr int kSlab = BN * BK * 2;  // one (tap, chunk) weight slab
     constexpr int kRowBytes = BK * 2;
-    constexpr int CW = BN < 32 ? BN : 32;
     static_assert(BN <= 64, "resident-weight variant is for narrow layers");
     static_assert(!kHead || BN == 32, "fused head expects the 32-channel output block");
     constexpr bool kCM = patch_chmajor(BN, BK, kHead);
@@ -94,8 +96,7 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
     const uint32_t a_base = w_base + static_cast<uint32_t>(ntaps * kc) * kSlab;
     const uint32_t stg_base = a_base + static_cast<uint32_t>(stages * kc) * p.patch_stride;  // a stage = all chunks of one tile
     constexpr uint32_t kStgBytes = ((kPatchTileW * kTileH * BN * 2 + 1023) / 1024) * 1024;    // one staging tile per group
-    const uint32_t xb_base = stg_base + 2u * kStgBytes;
-    const uint32_t bar_base = xb_base + (kCM ? 0u : 2u * xbuf_bytes<32>());  // the channel-major form needs no transpose buffers
+    const uint32_t bar_base = stg_base + 2u * kStgBytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kPatchMaxStages + s); };
     const uint32_t w_bar = bar_base + 8u * (2 * kPatchMaxStages);
@@ -213,16 +214,18 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
         if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete before exit
     } else {
         // ============ consumer warpgroups (MMA + epilogue), alternating tiles: group g takes tiles g, g+2, .. ============
+        // Fragment of m64nBNk16: warp q holds the GEMM rows 64h + 16q + lane/4 + 8r8 (h, r8 in {0,1}), i.e. tile pixel
+        // x = lane/4 of the rows 8h + 2q + r8 of the 8 x 16 tile, and in every 8-column chunk j the channel pair
+        // 8j + 2(lane%4) (acc[h][4j + 2r8 + {0,1}]).
         const int grp = (warp - 4) >> 2;
         const int q = (warp - 4) & 3;
-        const int row = q * 32 + lane;
-        const int py = row >> 3, px = row & 7;  // GEMM row -> pixel inside the 8 x 16 tile
+        const int px = lane >> 2;
+        const int cq = 2 * (lane & 3);
         const EpiParams& e = p.ep;
         constexpr uint32_t kOutRow = BN * 2;                                   // bytes per pixel in the staging tile
         constexpr uint32_t kOutSwz = (kOutRow == 128) ? 7u : (kOutRow == 64) ? 3u : 1u;   // matches tmO's swizzle mode
         constexpr uint32_t kInSwz = (BK == 64) ? 7u : (BK == 32) ? 3u : 1u;
         const uint32_t stg = stg_base + grp * kStgBytes;
-        float* const xb = reinterpret_cast<float*>(smem_raw + (xb_base - smem_raw_u32) + grp * xbuf_bytes<32>());
         const bool leader = (q == 0 && lane == 0);
         const uint32_t bar_id = 1 + grp;  // named barrier of this group (0 is __syncthreads)
         // Every tap is a shifted view of the patch: the 8 pixels of an output row are 8 consecutive patch rows (one 8-row
@@ -240,7 +243,6 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
             const int n = tile / tiles_per_img;
             const int r = tile - n * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-            const int x = tx * kPatchTileW + px, y = ty * kPatchTileH + py;
 
             mbar_wait(full_bar(stage), static_cast<uint32_t>(it / stages) & 1u);
             wg_fence();
@@ -257,39 +259,73 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
             wg_fence_regs<BN / 2>(acc[1]);
             if (p.res_row < 0 && lane == 0) mbar_arrive(empty_bar(stage));  // the MMAs were the patch's last readers
 
-            uint32_t v[BN];
+            // folded BatchNorm, the residual = this block's input = centre of the patch still resident in shared memory
+            // (K-major, swizzled by address bits exactly as TMA wrote it), the activation: all on the fragment
+            const uint32_t res = a_base + stage * kc * p.patch_stride + (p.res_row + px) * kRowBytes;
 #pragma unroll
-            for (int c0 = 0; c0 < BN; c0 += CW) acc_to_rows<CW>(acc[0], acc[1], c0, xb, bar_id, v + c0);
-            float f[BN];
+            for (int j = 0; j < BN / 8; ++j) {
+                const int cc = 8 * j + cq;
+                const float sc0 = p.cscale[cc], sc1 = p.cscale[cc + 1], sh0 = p.cshift[cc], sh1 = p.cshift[cc + 1];
 #pragma unroll
-            for (int j = 0; j < BN; ++j) f[j] = fmaf(__uint_as_float(v[j]), p.cscale[j], p.cshift[j]);
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int r8 = 0; r8 < 2; ++r8) {
+                        float* const a = &acc[h][4 * j + 2 * r8];
+                        a[0] = fmaf(a[0], sc0, sh0);
+                        a[1] = fmaf(a[1], sc1, sh1);
+                        if (p.res_row >= 0) {
+                            uint32_t ad = res + static_cast<uint32_t>((8 * h + 2 * q + r8) * p.PW) * kRowBytes + cc * 2;
+                            ad ^= ((ad >> 7) & kInSwz) << 4;
+                            uint32_t rv;
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rv) : "r"(ad));
+                            const float2 v = unpack2<kBF16>(rv);
+                            a[0] += v.x;
+                            a[1] += v.y;
+                        }
+                    }
+            }
             if (p.res_row >= 0) {
-                // residual = this block's input = centre of the patch still resident in shared memory (K-major,
-                // swizzled by address bits exactly as TMA wrote it)
-                const uint32_t prow = a_base + stage * kc * p.patch_stride + (p.res_row + py * p.PW + px) * kRowBytes;
-#pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    uint32_t a = prow + j * 16;
-                    a ^= ((a >> 7) & kInSwz) << 4;
-                    uint32_t r0, r1, r2, r3;
-                    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(a));
-                    const float2 a0 = unpack2<kBF16>(r0), a1 = unpack2<kBF16>(r1);
-                    const float2 a2 = unpack2<kBF16>(r2), a3 = unpack2<kBF16>(r3);
-                    f[8 * j + 0] += a0.x; f[8 * j + 1] += a0.y; f[8 * j + 2] += a1.x; f[8 * j + 3] += a1.y;
-                    f[8 * j + 4] += a2.x; f[8 * j + 5] += a2.y; f[8 * j + 6] += a3.x; f[8 * j + 7] += a3.y;
-                }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar(stage));  // this warp is done with the patch
             }
             if (e.act == ACT_RELU) {
 #pragma unroll
-                for (int j = 0; j < BN; ++j) f[j] = fmaxf(f[j], 0.0f);
+                for (int j = 0; j < BN / 2; ++j) { acc[0][j] = fmaxf(acc[0][j], 0.0f); acc[1][j] = fmaxf(acc[1][j], 0.0f); }
             } else if (e.act == ACT_LRELU) {
 #pragma unroll
-                for (int j = 0; j < BN; ++j) f[j] = f[j] > 0.0f ? f[j] : 0.01f * f[j];
+                for (int j = 0; j < BN / 2; ++j) {
+                    acc[0][j] = acc[0][j] > 0.0f ? acc[0][j] : 0.01f * acc[0][j];
+                    acc[1][j] = acc[1][j] > 0.0f ? acc[1][j] : 0.01f * acc[1][j];
+                }
             }
             if constexpr (kHead) {
-                // wav2lip.py:84-85: Conv2d(32,3,1) + Sigmoid on the fp32 block output still in registers
+                // wav2lip.py:84-85: Conv2d(32,3,1) + Sigmoid on the fp32 block output still in registers.  The four lanes of
+                // a quad hold the same four pixels (rows (h, r8)) and each 8 of their 32 channels; a two-step butterfly
+                // inside the quad gives lane t = 2h + r8 all 32 channels of row (h, r8), so each thread finishes one pixel
+                // with the dot products in channel order.
+                const int lh = (lane >> 1) & 1, lr = lane & 1;  // quad lane = 2 lh + lr holds pixel row (lh, lr)
+                float z[2][2][8];  // after the xor-2 step: z[s][r8][2j + e] = channel 8j + 2(2s + lr) + e of row (lh, r8)
+#pragma unroll
+                for (int r8 = 0; r8 < 2; ++r8)
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int k = 4 * (i >> 1) + 2 * r8 + (i & 1);
+                        const float recv = __shfl_xor_sync(0xffffffffu, lh ? acc[0][k] : acc[1][k], 2);
+                        z[0][r8][i] = lh ? recv : acc[0][k];
+                        z[1][r8][i] = lh ? acc[1][k] : recv;
+                    }
+                float f[32];
+#pragma unroll
+                for (int sh = 0; sh < 2; ++sh)
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const float recv = __shfl_xor_sync(0xffffffffu, lr ? z[sh][0][i] : z[sh][1][i], 1);
+                        // source lane (sh, sb) holds channels 8j + 2(2 sh + sb) + e of chunk j = i / 2, e = i % 2
+                        const int c0 = 8 * (i >> 1) + 2 * (2 * sh) + (i & 1);
+                        f[c0] = lr ? recv : z[sh][0][i];
+                        f[c0 + 2] = lr ? z[sh][1][i] : recv;
+                    }
+                const int x = tx * kPatchTileW + px, y = ty * kPatchTileH + 8 * lh + 2 * q + lr;
                 if (x < e.Wout && y < e.Hout) {
                     const int hb = n % e.head_B, ht = n / e.head_B;
                     const long long plane = (long long)e.Hout * e.Wout;
@@ -308,19 +344,20 @@ __global__ void __launch_bounds__(kPatchThreads, 1) conv_patch_kernel(const __gr
             } else {
                 // stage the tile (pixel-major rows of BN 16-bit channels, hardware swizzle pattern) and TMA-store it
                 if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous store has read the buffer
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+                named_bar_sync(bar_id, 128);
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    uint32_t a = stg + row * kOutRow + j * 16;
-                    a ^= ((a >> 7) & kOutSwz) << 4;
-                    const uint32_t o0 = pack2<kBF16>(f[8 * j + 0], f[8 * j + 1]);
-                    const uint32_t o1 = pack2<kBF16>(f[8 * j + 2], f[8 * j + 3]);
-                    const uint32_t o2 = pack2<kBF16>(f[8 * j + 4], f[8 * j + 5]);
-                    const uint32_t o3 = pack2<kBF16>(f[8 * j + 6], f[8 * j + 7]);
-                    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a), "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
-                }
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int r8 = 0; r8 < 2; ++r8) {
+                            uint32_t a = stg + (64 * h + 16 * q + 8 * r8 + px) * kOutRow + (8 * j + cq) * 2;
+                            a ^= ((a >> 7) & kOutSwz) << 4;
+                            const uint32_t o = pack2<kBF16>(acc[h][4 * j + 2 * r8], acc[h][4 * j + 2 * r8 + 1]);
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(o) : "memory");
+                        }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA engine
-                asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+                named_bar_sync(bar_id, 128);
                 if (leader) {
                     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                                  ::"l"(reinterpret_cast<uint64_t>(&p.tmO)), "r"(stg), "r"(0), "r"(tx * kPatchTileW), "r"(ty * kPatchTileH), "r"(n)

@@ -121,10 +121,10 @@ static int encode_w_map(w2l_ctx* ctx, CUtensorMap* tm, const PackedW& w, int BK,
 }
 
 // Few-channel stride-1 layers: one input patch per tile + resident weights (conv_patch.cuh)
-struct PatchGeom { int ox, oy, PW, PH, BK, TH, patch_bytes, patch_stride, wbytes, stg_bytes, xbuf_bytes, res_tap; };
+struct PatchGeom { int ox, oy, PW, PH, BK, TH, patch_bytes, patch_stride, wbytes, stg_bytes, res_tap; };
 
-// weights + patch ring + staging; the transpose buffers of the row-per-thread form and the barriers come on top
-static int patch_smem_budget(const PatchGeom& g) { return kSmemMax - kSmemExtra - g.xbuf_bytes; }
+// weights + patch ring + staging; the barriers come on top
+constexpr int kPatchSmemBudget = kSmemMax - kSmemExtra;
 
 static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) {
     if (!ctx->use_patch) return false;
@@ -136,10 +136,8 @@ static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) 
     if (a.Wl < kPatchTileW || a.Hl < kPatchTileW) return false;
     if (a.out.f32) return false;
     g->BK = pick_bk(w.cin_pad);
-    // the 64 -> 64 form runs channel-major on 8 x 32 tiles and needs no transpose buffers (conv_patch.cuh)
-    const bool chm = patch_chmajor(a.cout, g->BK, a.head);
-    g->TH = chm ? kChTileH : kPatchTileH;
-    g->xbuf_bytes = chm ? 0 : 2 * xbuf_bytes<32>();
+    // the 64 -> 64 form runs channel-major on 8 x 32 tiles (conv_patch.cuh)
+    g->TH = patch_chmajor(a.cout, g->BK, a.head) ? kChTileH : kPatchTileH;
     const double tiles = (double)((a.Wl + kPatchTileW - 1) / kPatchTileW) * ((a.Hl + g->TH - 1) / g->TH);
     if ((double)a.Wl * a.Hl / (tiles * kPatchTileW * g->TH) < 0.6) return false;
     int mnx = 127, mxx = -127, mny = 127, mxy = -127;
@@ -154,7 +152,7 @@ static bool patch_eligible(const w2l_ctx* ctx, const ConvArgs& a, PatchGeom* g) 
     g->wbytes = w.ntaps * w.cin_pad * a.cout * 2;
     g->stg_bytes = 2 * ((kPatchTileW * g->TH * a.cout * 2 + 1023) / 1024 * 1024);  // the kernel always carves two staging tiles
     if (g->PW > 256 || g->PH > 256) return false;
-    if (g->wbytes + g->stg_bytes + 2 * (w.cin_pad / g->BK) * g->patch_stride > patch_smem_budget(*g)) return false;
+    if (g->wbytes + g->stg_bytes + 2 * (w.cin_pad / g->BK) * g->patch_stride > kPatchSmemBudget) return false;
     g->res_tap = -1;
     if (a.res) {
         // the patch kernel takes the residual from the input patch in shared memory: it must BE the block input
@@ -188,8 +186,8 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     h.patch_bytes = g.patch_bytes; h.patch_stride = g.patch_stride;
     for (int t = 0; t < w.ntaps; ++t) h.tap_row[t] = (w.dy[t] - g.oy) * g.PW + (w.dx[t] - g.ox);
     // even: the two consumer warpgroups take alternate tiles, so each stage always goes to the same one
-    h.stages = std::min(kPatchMaxStages, (patch_smem_budget(g) - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride)) & ~1;
-    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + g.xbuf_bytes + kSmemExtra;
+    h.stages = std::min(kPatchMaxStages, (kPatchSmemBudget - g.wbytes - g.stg_bytes) / (h.kc * g.patch_stride)) & ~1;
+    op.dyn_smem = g.wbytes + h.stages * h.kc * g.patch_stride + g.stg_bytes + kSmemExtra;
     if (op.dyn_smem > kSmemMax || h.stages < 2) return fail(W2L_EINVAL, "%s: patch kernel smem plan %d B / %d stages", a.name.c_str(), op.dyn_smem, h.stages);
     fill_epi(&h.ep, a);
     h.res_row = g.res_tap >= 0 ? h.tap_row[g.res_tap] : -1;
@@ -388,7 +386,7 @@ static int make_convt_fused_op(w2l_ctx* ctx, Plan* pl, const Layer& L, const Lay
     t.patch_bytes = kCtPW * kCtPH * BK * 2;
     t.patch_stride = (t.patch_bytes + 1023) / 1024 * 1024;
     const int stage_bytes = t.patch_stride + 9 * kCtBN * BK * 2;
-    const int fixed = 2 * kTileM * kCtBN * 2 + 2 * xbuf_bytes<16>() + kSmemExtra;
+    const int fixed = 2 * kTileM * kCtBN * 2 + kSmemExtra;  // two staging tiles, alignment slack + barriers
     t.stages = std::min(kCtMaxStages, (kCtSmemMax - fixed) / stage_bytes);
     if (t.stages < 2) return fail(W2L_EINVAL, "%s: fused convT does not fit shared memory", L.name.c_str());
     op.dyn_smem = t.stages * stage_bytes + fixed;

@@ -129,13 +129,14 @@ static int load_layer(w2l_ctx* ctx, LayerW* lw, const Layer& L, const float* W, 
                 lw->ph.push_back(pw);
             }
         if (!ctx->x2 && L.cout == kCtBN && L.kh == 3 && L.kw == 3 && L.sh == 2 && L.sw == 2 && L.ph == 1 && L.pw == 1 && L.out_pad == 1) {
-            // all nine taps for the fused four-phase kernel, grouped by the input shift (dy,dx) they read and, inside a
-            // group, in the accumulator's phase order [00 | 01 | 11 | 10] (convt_fused.cuh): tap (r,s) belongs to phase
-            // ((r+1)&1, (s+1)&1) and reads in[y + (r==0), x + (s==0)]
-            std::vector<std::pair<int, int>> rs = {{1, 1}, {1, 2}, {2, 2}, {2, 1},   // shift (0,0): phases 00 01 11 10
-                                                   {1, 0}, {2, 0},                   // shift (0,1): phases 01 11
-                                                   {0, 2}, {0, 1},                   // shift (1,0): phases 11 10
-                                                   {0, 0}};                          // shift (1,1): phase 11
+            // all nine taps for the fused four-phase kernel in the slab order of its two consumer warpgroups
+            // (convt_fused.cuh): shift (0,0) for the accumulator's phase order [00 | 11 | 01 | 10] (each group's half one
+            // contiguous 128-column window), then the other taps of group 0's phase 11, then those of group 1's phases
+            // 01 and 10.  Tap (r,s) belongs to phase ((r+1)&1, (s+1)&1) and reads in[y + (r==0), x + (s==0)]
+            std::vector<std::pair<int, int>> rs = {{1, 1}, {2, 2}, {1, 2}, {2, 1},   // shift (0,0): phases 00 11 01 10
+                                                   {2, 0}, {0, 2}, {0, 0},           // phase 11: shifts (0,1) (1,0) (1,1)
+                                                   {1, 0},                           // phase 01: shift (0,1)
+                                                   {0, 1}};                          // phase 10: shift (1,0)
             PackedW pw;
             for (int t = 0; t < 9; ++t) { pw.dy.push_back(0); pw.dx.push_back(0); }
             CKR(pack_taps(ctx, lw, &pw, W, L.cout, L.cin, L.kh, L.kw, true, rs, pad_to, log, st));
