@@ -317,6 +317,45 @@ int w2l_stream_finish(w2l_stream* s, uint8_t* out_dev, int64_t cap, int64_t* fir
                       void* stream);
 int w2l_stream_destroy(w2l_stream* s);
 
+/* Stream group: many streaming sessions (each as w2l_stream_*: the loop of inference.py:224-244, :87-103, :120-140 and
+ * :259-271 on audio that arrives in pieces) sharing one context, one caller stream and one set of generator steps.  A
+ * tick takes the new audio of any subset of the sessions (and may finish some); it computes every row that audio fixes
+ * within the tick, pooled across sessions into as few steps as possible: full max_batch steps, then the rest in the
+ * smallest bucket (a power of two below max_batch, or max_batch) that holds it.  Each session's output equals a lone
+ * w2l_stream (and the offline loop) fed the same pieces, bit for bit.  Per tick the host makes one upload copy, one
+ * audio scatter and one mel launch, one NaN read-back (its only wait, apart from reusing a table staging slot), and per
+ * step one table copy and one graph launch, however many sessions take part.
+ *   _create: max_batch 1..4096; audio_ring_log2 as w2l_melstream_create (0 = 16).  The generator weights must be
+ *     loaded; new ones may be loaded between ticks.  The group must be destroyed before its context.
+ *   _open: frames_dev, d and rects_host as w2l_stream_create; *session_id gets the session's id.
+ *   _close: the session's rings are released (waits for the device).
+ *   _pending (host only): for each named session, the frames a tick with n_samples more (and finish) would emit.
+ *   _tick: n sessions ids[i] with pcm[i] (n_samples[i] fp32 16 kHz samples, host or device memory; pcm may be null
+ *     when every n_samples is 0) and finish[i] (finish may be null); frames go to out_dev[i] (cap[i] frames of
+ *     (H, W, 3) uint8), output indices first_index[i] .. + n_out[i] - 1.  Every argument, pointer and row is checked
+ *     before anything is launched; a bad one fails the whole tick (W2L_EINVAL / W2L_ESTATE) with nothing done.  A mel
+ *     frame holding a NaN fails its session only: status[i] = W2L_EINVAL, its rows of the tick are not run, and so on
+ *     for every later tick that names it; w2l_stream_group_error gives the reference's message (inference.py:228-229),
+ *     "" for a session that has not failed.  The return code is for group-wide errors.
+ *   _buckets (host only, no context): the bucket of each step that n_rows pooled rows take; returns the step count and
+ *     writes the first cap sizes.
+ *   _counters: CUDA API submissions (launches, graph launches, copies, event records and waits), host waits and steps
+ *     made by all ticks so far (any may be null). */
+typedef struct w2l_stream_group w2l_stream_group;
+int w2l_stream_group_create(w2l_ctx* ctx, int max_batch, int audio_ring_log2, w2l_stream_group** out);
+int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
+                          const int32_t* rects_host, int32_t* session_id);
+int w2l_stream_group_close(w2l_stream_group* g, int32_t session_id);
+int w2l_stream_group_pending(const w2l_stream_group* g, int n, const int32_t* ids, const int64_t* n_samples,
+                             const int32_t* finish, int64_t* n_out);
+int w2l_stream_group_tick(w2l_stream_group* g, int n, const int32_t* ids, const float* const* pcm,
+                          const int64_t* n_samples, const int32_t* finish, uint8_t* const* out_dev, const int64_t* cap,
+                          int64_t* first_index, int64_t* n_out, int32_t* status, void* stream);
+const char* w2l_stream_group_error(const w2l_stream_group* g, int32_t session_id);
+int w2l_stream_group_buckets(int max_batch, int64_t n_rows, int32_t* sizes, int64_t cap);
+int w2l_stream_group_counters(const w2l_stream_group* g, int64_t* calls, int64_t* host_waits, int64_t* steps);
+int w2l_stream_group_destroy(w2l_stream_group* g);
+
 /* ---- test aids ---- */
 /* keep every block output of subsequent plans addressable (no buffer reuse) for w2l_debug_layer_output */
 int w2l_set_debug(w2l_ctx* ctx, int keep_all_layer_outputs);

@@ -37,6 +37,17 @@ with torch.no_grad():
     sess = LipSyncSession(g, frames, 25.0, rects=[(7, 5, 80, 60), (0, 0, 88, 62)], batch=2)
     sfr = [sess.push(np.random.randn(3200).astype(np.float32))[1] for _ in range(3)] + [sess.finish()[1]]
     sess.close()
+    # a stream group: the audio scatter (host and device pieces), the multi-ring mel kernel, and steps of two bucket
+    # sizes (a padding row, frames of two sizes, one not 16-byte aligned) uncaptured and replayed
+    from wav2lip_b200.stream import LipSyncServer
+    srv = LipSyncServer(g, max_batch=4, audio_ring_log2=11)
+    frames2 = torch.randint(0, 256, (3, 57, 91, 3), dtype=torch.uint8).cuda()
+    ga = srv.open(frames, 25.0, rects=[(7, 5, 80, 60), (0, 0, 88, 62)])
+    gb = srv.open(frames2, 29.97, box=(3, 50, 5, 80))
+    gw = np.random.randn(9000).astype(np.float32)
+    gfr = [srv.tick({ga: gw[k:k + 1500], gb: torch.from_numpy(gw[k:k + 1500]).cuda()}) for k in range(0, 6000, 1500)]
+    gfr.append(srv.tick({ga: gw[6000:]}, finish=[ga, gb]))
+    srv.close()
     # many units of 128-channel tiles: a 128-channel residual block and a transposed-conv phase set
     from wav2lip_b200.models.conv import Conv2d, Conv2dTranspose
     sw = Conv2d(128, 128, 3, 1, 1, residual=True).cuda().eval()(torch.rand(140, 128, 24, 24).cuda())

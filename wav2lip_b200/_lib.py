@@ -38,6 +38,9 @@ EXPORTS = [
     "w2l_melstream_create", "w2l_melstream_pending", "w2l_melstream_push", "w2l_melstream_finish", "w2l_melstream_destroy",
     "w2l_stream_schedule", "w2l_stream_create", "w2l_stream_pending", "w2l_stream_push", "w2l_stream_finish",
     "w2l_stream_destroy",
+    "w2l_stream_group_create", "w2l_stream_group_open", "w2l_stream_group_close", "w2l_stream_group_pending",
+    "w2l_stream_group_tick", "w2l_stream_group_error", "w2l_stream_group_buckets", "w2l_stream_group_counters",
+    "w2l_stream_group_destroy",
 ]
 STREAM_ROW = 7  # W2L_STREAM_ROW: output index, chunk start, frame index, y1, y2, x1, x2
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
@@ -203,6 +206,16 @@ def get_lib() -> C.CDLL:
     lib.w2l_stream_push.argtypes = [vp, vp, i64, vp, i64, pi64, pi64, vp]
     lib.w2l_stream_finish.argtypes = [vp, vp, i64, pi64, pi64, vp]
     lib.w2l_stream_destroy.argtypes = [vp]
+    lib.w2l_stream_group_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
+    lib.w2l_stream_group_open.argtypes = [vp, vp, C.POINTER(StreamDesc), vp, C.POINTER(i32)]
+    lib.w2l_stream_group_close.argtypes = [vp, i32]
+    lib.w2l_stream_group_pending.argtypes = [vp, i32, vp, vp, vp, vp]
+    lib.w2l_stream_group_tick.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.w2l_stream_group_error.argtypes = [vp, i32]
+    lib.w2l_stream_group_error.restype = cp
+    lib.w2l_stream_group_buckets.argtypes = [i32, i64, vp, i64]
+    lib.w2l_stream_group_counters.argtypes = [vp, pi64, pi64, pi64]
+    lib.w2l_stream_group_destroy.argtypes = [vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here == header / library mismatch
     if lib.w2l_abi_version() != 1:

@@ -295,4 +295,24 @@ __global__ void __launch_bounds__(MEL_THREADS, 4) mel_ring_kernel(const MelParam
     mel_frames(p, MelRingSrc{r.audio, r.audio_mask, r.L}, MelRingDst{r.mel, r.mel_pitch, r.nan}, r.f0, r.f1);
 }
 
+// ---- many rings in one launch (w2l_stream_group_*): block b computes up to MEL_FPB frames of one session ----
+// Each block reads its own descriptor, so one launch covers every session of a tick however few frames each has.  The
+// body indexes frames from f0 + blockIdx.x * MEL_FPB; passing f0 = fb - blockIdx.x * MEL_FPB leaves that indexing, and
+// with it the instruction sequence of mel_kernel and mel_ring_kernel, as it was.
+struct MelGroupBlock {
+    const float* audio;
+    long long audio_mask;
+    float* mel;
+    long long mel_pitch;
+    long long L;          // see MelRingSrc::L
+    long long fb, f1;     // frames [fb, min(fb + MEL_FPB, f1))
+    int* nan;             // the session's sticky flag
+};
+
+__global__ void __launch_bounds__(MEL_THREADS, 4) mel_group_kernel(const MelParams p, const MelGroupBlock* blocks) {
+    const MelGroupBlock b = blocks[blockIdx.x];
+    mel_frames(p, MelRingSrc{b.audio, b.audio_mask, b.L}, MelRingDst{b.mel, b.mel_pitch, b.nan},
+               b.fb - (long long)blockIdx.x * MEL_FPB, b.f1);
+}
+
 }  // namespace w2l

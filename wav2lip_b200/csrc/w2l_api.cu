@@ -43,6 +43,7 @@ using namespace w2l;
 #include "host_mel_tables.h"
 #include "host_train.cuh"
 #include "host_stream.cuh"
+#include "host_stream_group.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // C-ABI

@@ -181,3 +181,165 @@ class LipSyncSession:
             self.close()
         except Exception:
             pass
+
+
+class LipSyncServer:
+    """Many streaming sessions over one `model`, sharing its context, the caller's stream and the generator steps
+    (include/w2l.h `w2l_stream_group_*`, DESIGN.md section 3.9).  Each session gives the same frames as a lone
+    `LipSyncSession` fed the same pieces, and as the offline loop, bit for bit.
+
+        srv = LipSyncServer(model, max_batch=128)
+        a = srv.open(frames_a, 25.0, rects=rects_a)             # the arguments of LipSyncSession, without batch
+        b = srv.open(frames_b, 29.97, box=(y1, y2, x1, x2))
+        out = srv.tick({a: pcm_a, b: pcm_b}, finish=[b])       # {session: (first_index, (n, H, W, 3) uint8 CUDA tensor)}
+        srv.close(a)
+
+    A tick runs every row its audio fixes, pooled across the sessions it names: full `max_batch` steps, then the rest in
+    the smallest power-of-two bucket that holds it.  A session whose audio gives a NaN mel frame fails alone: `tick`
+    returns the `ValueError` (the reference's message) as that session's value instead of raising, the other sessions'
+    frames are returned as usual, and every later tick that names the failed session raises that `ValueError` before
+    anything runs.  A bad argument raises before anything runs, for the whole tick.  `audio_ring_log2` sets the audio
+    ring of every session (0: 2^16 samples)."""
+
+    def __init__(self, model, max_batch=128, audio_ring_log2=0):
+        if isinstance(max_batch, bool) or int(max_batch) != max_batch or int(max_batch) < 1:
+            raise ValueError(f"max_batch must be a positive integer, got {max_batch!r}")
+        self.model = model
+        self.max_batch = int(max_batch)
+        self._ring_log2 = int(audio_ring_log2)
+        self._h = None
+        self._ctx = None
+        self._sessions = {}   # id -> (frames, (H, W))
+        self._failed = {}     # id -> message
+
+    def _group(self, frames):
+        ctx = self.model._ensure(frames)   # reloads the weights if the model's parameters changed
+        if self._h is None:
+            h = C.c_void_p()
+            _raise(ctx.lib.w2l_stream_group_create(ctx.h, self.max_batch, self._ring_log2, C.byref(h)))
+            self._h, self._ctx, self._lib = h, ctx, ctx.lib
+        elif ctx is not self._ctx:
+            raise L.W2LError("the model moved to another device or context since the server was created")
+        return ctx
+
+    def open(self, frames_u8, fps, rects=None, pads=(0, 10, 0, 0), nosmooth=False, box=None):
+        """A new session -> its id (an int)."""
+        if not isinstance(frames_u8, torch.Tensor) or not frames_u8.is_cuda:
+            raise L.W2LError("frames_u8 must be a CUDA tensor: wav2lip_b200 has no CPU path")
+        if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[3] != 3 or frames_u8.shape[0] < 1:
+            raise ValueError(f"expected uint8 (F,H,W,3) frames, got {frames_u8.dtype} {tuple(frames_u8.shape)}")
+        if not (float(fps) > 0) or not np.isfinite(float(fps)):
+            raise ValueError(f"fps must be positive and finite, got {fps!r}")
+        if rects is None and box is None:
+            raise ValueError("pass the detector rects of every frame or one fixed box")
+        F, H, W = (int(v) for v in frames_u8.shape[:3])
+        desc = _desc(F, H, W, fps, pads, nosmooth, box)
+        ra = _rects_array(rects, F) if box is None else None
+        frames = frames_u8.contiguous()
+        ctx = self._group(frames)
+        self.model._same_device(ctx, frames)
+        sid = C.c_int32()
+        _raise(self._lib.w2l_stream_group_open(self._h, C.c_void_p(frames.data_ptr()), C.byref(desc),
+                                               ra.ctypes.data_as(C.c_void_p) if ra is not None else None, C.byref(sid)))
+        self._sessions[sid.value] = (frames, (H, W))
+        return sid.value
+
+    def tick(self, pieces, finish=()):
+        """pieces: {session: float32 16 kHz samples (host or CUDA), or None}; finish: sessions whose utterance ends
+        with this tick (they may be absent from pieces) -> {session: (first_index, frames)} for every session named."""
+        if self._h is None:
+            raise L.W2LError("no session is open")
+        ids = list(pieces.keys()) + [s for s in finish if s not in pieces]
+        fin = set(finish)
+        for s in ids:
+            if s not in self._sessions:
+                raise L.W2LError(f"session {s!r} is not open in this server")
+            if s in self._failed:
+                raise ValueError(self._failed[s])
+        frames0 = self._sessions[ids[0]][0] if ids else None
+        if frames0 is not None and self._group(frames0) is not self._ctx:
+            raise L.W2LError("the model moved to another device or context since the server was created")
+        n = len(ids)
+        dev = frames0.device if n else None
+        keep, ptrs, counts = [], (C.c_void_p * max(n, 1))(), (C.c_int64 * max(n, 1))()
+        for i, s in enumerate(ids):
+            pcm = pieces.get(s)
+            if pcm is None:
+                continue
+            if isinstance(pcm, torch.Tensor) and pcm.is_cuda:
+                if pcm.device != dev:
+                    raise ValueError(f"pcm is on {pcm.device}, the server on {dev}")
+                k = pcm.detach().reshape(-1).contiguous().float()
+                ptrs[i], counts[i] = k.data_ptr(), k.numel()
+            else:
+                x = pcm.detach().cpu().numpy() if isinstance(pcm, torch.Tensor) else pcm
+                k = np.ascontiguousarray(np.asarray(x, dtype=np.float32).reshape(-1))
+                ptrs[i], counts[i] = k.ctypes.data, k.shape[0]
+            keep.append(k)
+        ids_a = (C.c_int32 * max(n, 1))(*ids)
+        fin_a = (C.c_int32 * max(n, 1))(*[1 if s in fin else 0 for s in ids])
+        need = (C.c_int64 * max(n, 1))()
+        _raise(self._lib.w2l_stream_group_pending(self._h, n, ids_a, counts, fin_a, need))
+        # one flat output buffer, a view per session
+        sizes = [need[i] * self._sessions[s][1][0] * self._sessions[s][1][1] * 3 for i, s in enumerate(ids)]
+        flat = torch.empty(max(sum(sizes), 1), device=dev, dtype=torch.uint8) if n else None
+        outs, optrs, at = [], (C.c_void_p * max(n, 1))(), 0
+        for i, s in enumerate(ids):
+            H, W = self._sessions[s][1]
+            outs.append(flat[at:at + sizes[i]].view(need[i], H, W, 3))
+            optrs[i] = flat.data_ptr() + at if need[i] else None
+            at += sizes[i]
+        first, got, status = (C.c_int64 * max(n, 1))(), (C.c_int64 * max(n, 1))(), (C.c_int32 * max(n, 1))()
+        stream = torch.cuda.current_stream(dev).cuda_stream if n else 0
+        _raise(self._lib.w2l_stream_group_tick(self._h, n, ids_a, ptrs, counts, fin_a, optrs, need, first, got, status,
+                                               C.c_void_p(stream)))
+        res = {}
+        for i, s in enumerate(ids):
+            if status[i] != L.W2L_OK:
+                msg = self._lib.w2l_stream_group_error(self._h, s).decode("utf-8", "replace")
+                self._failed[s] = msg
+                res[s] = ValueError(msg)
+                continue
+            assert got[i] == need[i]
+            res[s] = (int(first[i]), outs[i])
+        if any(got[i] for i in range(n)):
+            self.model._range_guard(self._ctx, stream)
+        return res
+
+    def counters(self):
+        """(CUDA API submissions, host waits, steps) of every tick so far."""
+        c, w, st = C.c_int64(), C.c_int64(), C.c_int64()
+        if self._h is not None:
+            _raise(self._lib.w2l_stream_group_counters(self._h, C.byref(c), C.byref(w), C.byref(st)))
+        return c.value, w.value, st.value
+
+    def close(self, session=None):
+        """Close one session, or (no argument) the whole server."""
+        if session is not None:
+            if session not in self._sessions:
+                raise L.W2LError(f"session {session!r} is not open in this server")
+            _raise(self._lib.w2l_stream_group_close(self._h, session))
+            del self._sessions[session]
+            self._failed.pop(session, None)
+            return
+        if self._h is not None:
+            self._lib.w2l_stream_group_destroy(self._h)
+            self._h = None
+        self._sessions.clear()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def stream_buckets(max_batch, n_rows):
+    """Host only (no GPU): the bucket size of each step that `n_rows` pooled rows take in a group of `max_batch`."""
+    lib = L.get_lib()
+    k = lib.w2l_stream_group_buckets(int(max_batch), int(n_rows), None, 0)
+    if k < 0:
+        _raise(k)
+    out = (C.c_int32 * max(k, 1))()
+    lib.w2l_stream_group_buckets(int(max_batch), int(n_rows), out, k)
+    return [int(out[i]) for i in range(k)]
