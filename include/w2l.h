@@ -297,6 +297,13 @@ typedef struct w2l_stream_desc {
 int w2l_stream_schedule(const w2l_stream_desc* d, const int32_t* rects_host, int64_t n_samples, int final_,
                         int64_t first_row, int64_t cap, int32_t* rows_host, int64_t* n_fixed);
 
+/* Pure host function: *n_frames gets need, the count of the prefix [0, need) of frames whose rects the rows that
+ * n_samples fix read (all rows of an utterance of n_samples with final != 0).  Rects of frames at or past need do not
+ * change those rows.  F == 1: 1.  nosmooth: the frames shown.  Smoothing: rows i read rects i .. i+4 while n_total is
+ * unknown, all of [0, n_total) once it is known.  At final it is n_total (inference.py:244, :113).  d must not have
+ * has_box; its rects are not needed. */
+int w2l_stream_detect_need(const w2l_stream_desc* d, int64_t n_samples, int final_, int64_t* n_frames);
+
 /* Every step runs the generator at exactly `batch` rows (one plan; rows past the ready ones repeat the last ready row
  * and are dropped), from a CUDA graph captured once per session and replayed (W2L_DISABLE_STREAMGRAPH=1 launches the
  * same kernels directly).  The generator weights must be loaded; loading new ones between pushes is allowed.
@@ -328,6 +335,18 @@ int w2l_stream_destroy(w2l_stream* s);
  *   _create: max_batch 1..4096; audio_ring_log2 as w2l_melstream_create (0 = 16).  The generator weights must be
  *     loaded; new ones may be loaded between ticks.  The group must be destroyed before its context.
  *   _open: frames_dev, d and rects_host as w2l_stream_create; *session_id gets the session's id.
+ *   _open_detect: as _open without rects or box (d->has_box = 0): the group finds each frame's box with the S3FD weights
+ *     of its context (w2l_load_weights(ctx, W2L_NET_S3FD, ...); W2L_ESTATE without them), as
+ *     get_detections_for_batch_u8 does on inference.py's BGR frames (inference.py:68-103: reversed channels, the first
+ *     box, clipped at 0 and truncated), on a stream of the group's own.  Frames of at least 32 x 32, written by work
+ *     queued on the legacy default stream before the call (or complete).  Only the frames a tick's rows read are
+ *     detected (w2l_stream_detect_need), just before that tick needs them: _open queues the frames of the first 400 ms of
+ *     audio without waiting, each tick the frames its own audio needs that no launch covers yet, then those of 200 ms
+ *     more, and each tick's one host wait covers every launch queued before it.  Launches take up to 16 frames of one
+ *     size from any sessions; S3FD plans of batch 1, 4 and 16 per frame size stay pinned while a detecting session of
+ *     that size is open.  A frame a tick's rows need without a face (or with a non-finite box) fails its session as a
+ *     NaN does, with face_boxes' message (inference.py:91-93) or the non-finite box's, both naming the frame.  A frame
+ *     past the ones the utterance needs fails nothing.
  *   _close: the session's rings are released (waits for the device).
  *   _pending (host only): for each named session, the frames a tick with n_samples more (and finish) would emit.
  *   _tick: n sessions ids[i] with pcm[i] (n_samples[i] fp32 16 kHz samples, host or device memory; pcm may be null
@@ -345,6 +364,8 @@ typedef struct w2l_stream_group w2l_stream_group;
 int w2l_stream_group_create(w2l_ctx* ctx, int max_batch, int audio_ring_log2, w2l_stream_group** out);
 int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
                           const int32_t* rects_host, int32_t* session_id);
+int w2l_stream_group_open_detect(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
+                                 int32_t* session_id);
 int w2l_stream_group_close(w2l_stream_group* g, int32_t session_id);
 int w2l_stream_group_pending(const w2l_stream_group* g, int n, const int32_t* ids, const int64_t* n_samples,
                              const int32_t* finish, int64_t* n_out);

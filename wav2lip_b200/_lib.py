@@ -37,8 +37,9 @@ EXPORTS = [
     "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
     "w2l_melstream_create", "w2l_melstream_pending", "w2l_melstream_push", "w2l_melstream_finish", "w2l_melstream_destroy",
     "w2l_stream_schedule", "w2l_stream_create", "w2l_stream_pending", "w2l_stream_push", "w2l_stream_finish",
-    "w2l_stream_destroy",
-    "w2l_stream_group_create", "w2l_stream_group_open", "w2l_stream_group_close", "w2l_stream_group_pending",
+    "w2l_stream_destroy", "w2l_stream_detect_need",
+    "w2l_stream_group_create", "w2l_stream_group_open", "w2l_stream_group_open_detect", "w2l_stream_group_close",
+    "w2l_stream_group_pending",
     "w2l_stream_group_tick", "w2l_stream_group_error", "w2l_stream_group_buckets", "w2l_stream_group_counters",
     "w2l_stream_group_destroy",
 ]
@@ -201,6 +202,7 @@ def get_lib() -> C.CDLL:
     lib.w2l_melstream_finish.argtypes = [vp, vp, i64, pi64, C.POINTER(i32), vp]
     lib.w2l_melstream_destroy.argtypes = [vp]
     lib.w2l_stream_schedule.argtypes = [C.POINTER(StreamDesc), vp, i64, i32, i64, i64, vp, pi64]
+    lib.w2l_stream_detect_need.argtypes = [C.POINTER(StreamDesc), i64, i32, pi64]
     lib.w2l_stream_create.argtypes = [vp, vp, C.POINTER(StreamDesc), vp, i32, C.POINTER(vp)]
     lib.w2l_stream_pending.argtypes = [vp, i64, i32, pi64]
     lib.w2l_stream_push.argtypes = [vp, vp, i64, vp, i64, pi64, pi64, vp]
@@ -208,6 +210,7 @@ def get_lib() -> C.CDLL:
     lib.w2l_stream_destroy.argtypes = [vp]
     lib.w2l_stream_group_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     lib.w2l_stream_group_open.argtypes = [vp, vp, C.POINTER(StreamDesc), vp, C.POINTER(i32)]
+    lib.w2l_stream_group_open_detect.argtypes = [vp, vp, C.POINTER(StreamDesc), C.POINTER(i32)]
     lib.w2l_stream_group_close.argtypes = [vp, i32]
     lib.w2l_stream_group_pending.argtypes = [vp, i32, vp, vp, vp, vp]
     lib.w2l_stream_group_tick.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]

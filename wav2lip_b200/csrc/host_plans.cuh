@@ -367,6 +367,7 @@ struct S3fdRun {
     int max_det;
     float* dets;            // (B, max_det, 5)
     int32_t* counts;        // (B)
+    const uint8_t* const* frame_ptrs = nullptr;   // device table of B (H, W, 3) frames, read instead of `frames`
 };
 
 static int get_plan(w2l_ctx* ctx, int net, int B, int T, Plan** out, int H = 0, int W = 0) {
@@ -427,9 +428,13 @@ static int run_plan(w2l_ctx* ctx, Plan* pl, const void* in0, const void* in1, vo
                     sp.src = det->frames; sp.dst = op.ip.dst;
                     sp.N = op.ip.N; sp.H = op.ip.H; sp.W = op.ip.W; sp.Cpad = op.ip.Cpad; sp.Wp = op.ip.Wp; sp.x_off = op.ip.x_off;
                     sp.Cpix = op.ip.Cpix; sp.lo_off = op.ip.lo_off; sp.reverse = det->reverse;
+                    sp.srcs = det->frame_ptrs;
                     const long long tot = (long long)sp.N * sp.H * sp.W;
                     const int blk = (int)std::min<long long>((tot + 255) / 256, ctx->num_sms * 16);
-                    if (ctx->bf16) s3fd_ingest_u8_kernel<true><<<blk, 256, 0, st>>>(sp);
+                    if (det->frame_ptrs) {
+                        if (ctx->bf16) s3fd_ingest_u8_kernel<true, true><<<blk, 256, 0, st>>>(sp);
+                        else s3fd_ingest_u8_kernel<false, true><<<blk, 256, 0, st>>>(sp);
+                    } else if (ctx->bf16) s3fd_ingest_u8_kernel<true><<<blk, 256, 0, st>>>(sp);
                     else s3fd_ingest_u8_kernel<false><<<blk, 256, 0, st>>>(sp);
                     ctx->launches++;
                     break;

@@ -163,28 +163,32 @@ struct StreamSched {
         bool final = false;
     };
 
-    int init(const w2l_stream_desc* desc, const int32_t* rects) {
+    // detect: the rects arrive frame by frame through set_rect (rects unused, d.has_box must be 0)
+    int init(const w2l_stream_desc* desc, const int32_t* rects, bool detect = false) {
         if (!desc) return fail(W2L_EINVAL, "null stream description");
         d = *desc;
         if (d.F < 1 || d.H < 1 || d.W < 1) return fail(W2L_EINVAL, "bad video shape F=%d H=%d W=%d", d.F, d.H, d.W);
         if (!(d.fps > 0) || !std::isfinite(d.fps)) return fail(W2L_EINVAL, "fps must be positive and finite (got %g)", d.fps);
         mult = 80. / d.fps;
+        if (detect && d.has_box) return fail(W2L_EINVAL, "a fixed box and face detection exclude each other");
         if (d.has_box) {
             const int32_t* b = d.box;
             if (b[0] < 0 || b[1] > d.H || b[0] >= b[1] || b[2] < 0 || b[3] > d.W || b[2] >= b[3])
                 return fail(W2L_EINVAL, "box (y %d:%d, x %d:%d) is empty or outside the %dx%d frame", b[0], b[1], b[2], b[3], d.H, d.W);
             return W2L_OK;
         }
-        if (!rects) return fail(W2L_EINVAL, "neither detector rects nor a fixed box");
-        padded.resize((size_t)d.F * 4);
-        for (int j = 0; j < d.F; ++j) {
-            const int32_t* r = rects + 4 * j;
-            padded[4 * j + 0] = std::max(0, r[0] - d.pads[2]);
-            padded[4 * j + 1] = std::max(0, r[1] - d.pads[0]);
-            padded[4 * j + 2] = std::min(d.W, r[2] + d.pads[3]);
-            padded[4 * j + 3] = std::min(d.H, r[3] + d.pads[1]);
-        }
+        if (!rects && !detect) return fail(W2L_EINVAL, "neither detector rects nor a fixed box");
+        padded.assign((size_t)d.F * 4, 0);
+        if (!detect)
+            for (int j = 0; j < d.F; ++j) set_rect(j, rects + 4 * j);
         return W2L_OK;
+    }
+
+    void set_rect(long long j, const int32_t* r) {
+        padded[4 * j + 0] = std::max(0, r[0] - d.pads[2]);
+        padded[4 * j + 1] = std::max(0, r[1] - d.pads[0]);
+        padded[4 * j + 2] = std::min(d.W, r[2] + d.pads[3]);
+        padded[4 * j + 3] = std::min(d.H, r[3] + d.pads[1]);
     }
 
     long long start(long long i) const { return (long long)((double)i * mult); }
@@ -216,6 +220,18 @@ struct StreamSched {
         // otherwise output i shows frame i, whose smoothed box is final once i + 5 <= n_lb
         a->n_fixed = box_now ? n_reg : std::max(0LL, std::min(n_reg, n_lb - 4));
         return W2L_OK;
+    }
+
+    // The frames whose rects rows [0, a.n_fixed) read: always a prefix [0, need).  F == 1: frame 0.  nosmooth: the
+    // frames shown.  Smoothing: the padded rows i .. i+4 of each row i while n_total is unknown (n_fixed + 4 <= n_lb < F),
+    // all of [0, n_total) once it is known (the tail window's in-place smoothing reads every earlier row).  At final this
+    // is n_total: the frames inference.py detects on (:244, :113), and none past them.
+    long long need(const At& a) const {
+        if (d.has_box) return 0;
+        if (d.F == 1) return 1;
+        if (a.n_fixed == 0) return 0;
+        if (d.nosmooth) return a.n_total >= 0 ? std::min(a.n_fixed, a.n_total) : a.n_fixed;
+        return a.n_total >= 0 ? a.n_total : a.n_fixed + 4;
     }
 
     const std::vector<long long>& smooth_first(long long n) {
@@ -584,6 +600,16 @@ int w2l_stream_schedule(const w2l_stream_desc* d, const int32_t* rects_host, int
     *n_fixed = a.n_fixed;
     for (long long i = first_row; i < a.n_fixed && i < first_row + cap; ++i)
         CKR(sc.row(i, a, rows_host + (size_t)(i - first_row) * W2L_STREAM_ROW));
+    return W2L_OK;
+}
+
+int w2l_stream_detect_need(const w2l_stream_desc* d, int64_t n_samples, int final_, int64_t* n_frames) {
+    if (!n_frames || n_samples < 0) return fail(W2L_EINVAL, "bad argument");
+    StreamSched sc;
+    CKR(sc.init(d, nullptr, true));
+    StreamSched::At a;
+    CKR(sc.at(n_samples, final_ != 0, &a));
+    *n_frames = sc.need(a);
     return W2L_OK;
 }
 

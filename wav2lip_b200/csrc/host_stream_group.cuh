@@ -18,6 +18,17 @@ static int group_bucket(int max_batch, long long n) {
     return std::min(b, max_batch);
 }
 
+// Face detection inside the group (DESIGN.md section 3.10).  Constants, not options: the detector batch of
+// inference.py's --face_det_batch_size default, and the look-ahead that lets a tick at real-time audio find the rects it
+// needs already read back.
+constexpr int kDetMaxBatch = 16;
+constexpr long long kDetOpenSamples = 6400;    // open: the frames the first 400 ms of audio need
+constexpr long long kDetAheadSamples = 3200;   // after a tick: the frames need(L + 200 ms) adds
+
+// S3FD batch of the next launch for r frames of one size: full 16s, a remainder above 8 as one 16, above 1 as 4s, else
+// 1.  Three plans per frame size; padding (the last frame repeated) is at most 7 frames.
+static int det_bucket(long long r) { return r > 8 ? 16 : r > 1 ? 4 : 1; }
+
 struct GroupSession {
     int32_t id = -1;
     int slot = 0;                    // its NaN flag: w2l_stream_group::nan[slot]
@@ -25,7 +36,12 @@ struct GroupSession {
     MelRing mel;
     const uint8_t* frames = nullptr;
     long long emitted = 0;           // rows whose step has been queued
-    bool nan = false, finished = false;
+    bool failed = false, finished = false;
+    std::string msg;                 // why it failed: the NaN message, or a detection's
+    bool detect = false;             // rects found by the group's detector
+    long long det_launched = 0;      // frames [0, det_launched) have a detection queued or read back
+    long long det_ok = 0;            // frames [0, det_ok) were read back with a face
+    std::vector<int8_t> det_status;  // per frame: -1 not read back yet, else kRectFace / kRectNone / kRectNonFinite
     long long first_lo = -1;         // the lowest mel frame of its first step
     long long trk_step[kGroupTrack], trk_lo[kGroupTrack];   // its last steps, oldest first
     int n_trk = 0;
@@ -60,6 +76,25 @@ struct GroupBucket {
     bool warm = false;               // one uncaptured step ran on the current plan (kernel attributes are set)
 };
 
+// an S3FD plan of one (H, W, B), pinned while a detecting session of that frame size is open; valid while epoch matches
+struct DetPlan {
+    int H = 0, W = 0, B = 0;
+    Plan* plan = nullptr;
+    uint64_t epoch = 0;
+};
+
+// One detection launch: up to kDetMaxBatch frames of one size.  Device block: [frame pointers][dets (B, 1, 5) fp32]
+// [counts][rects (B, 5) int32]; pinned block: [frame pointers][rects].
+constexpr size_t kDetDevPtrs = 0, kDetDevDets = 128, kDetDevCounts = 448, kDetDevRects = 512, kDetDevBytes = 832;
+constexpr size_t kDetHostRects = 128, kDetHostBytes = 448;
+struct DetJob {
+    int n = 0;                       // real frames (the rest repeat the last one)
+    int32_t sid[kDetMaxBatch];
+    int32_t frame[kDetMaxBatch];
+    DevMem<uint8_t> dev;
+    PinnedMem host;
+};
+
 struct w2l_stream_group {
     w2l_ctx* ctx = nullptr;
     int max_batch = 0, ring_log2 = 0;
@@ -92,7 +127,140 @@ struct w2l_stream_group {
     Stream cap;                      // capture stream
     int64_t calls = 0, waits = 0;    // CUDA API submissions (launches, graph launches, copies, event records and waits)
                                      // and host synchronisations made by ticks
+    // Face detection runs on a stream of its own; ev_det follows the last launch.  Every launch is read back by the
+    // next round's host wait (the mel stream waits for ev_det before its NaN read-back), so jobs are busy until then.
+    Stream s_det;
+    Event ev_det, ev_open;
+    std::vector<std::unique_ptr<DetJob>> det_busy, det_free;
+    std::vector<DetPlan> det_plans;
+    std::map<std::pair<int, int>, int> det_sizes;   // open detecting sessions per (H, W)
 };
+
+static void group_det_release(w2l_stream_group* g, int H, int W) {
+    auto& v = g->det_plans;
+    for (DetPlan& p : v)
+        if (p.H == H && p.W == W && p.plan && p.epoch == g->ctx->plan_epoch[W2L_NET_S3FD]) p.plan->pins--;
+    v.erase(std::remove_if(v.begin(), v.end(), [&](const DetPlan& p) { return p.H == H && p.W == W; }), v.end());
+}
+
+// the S3FD plan of (H, W, B), pinned; after new weights (drop_plans) the old one is gone and a new one is taken
+static int group_det_plan(w2l_stream_group* g, int H, int W, int B, Plan** out) {
+    w2l_ctx* ctx = g->ctx;
+    size_t k = 0;
+    while (k < g->det_plans.size() && !(g->det_plans[k].H == H && g->det_plans[k].W == W && g->det_plans[k].B == B)) ++k;
+    if (k < g->det_plans.size() && g->det_plans[k].plan && g->det_plans[k].epoch == ctx->plan_epoch[W2L_NET_S3FD]) {
+        *out = g->det_plans[k].plan;
+        return W2L_OK;
+    }
+    if (k == g->det_plans.size()) {
+        DetPlan p;
+        p.H = H; p.W = W; p.B = B;
+        g->det_plans.push_back(p);
+    }
+    g->det_plans[k].plan = nullptr;
+    Plan* pl;
+    CKR(get_plan(ctx, W2L_NET_S3FD, B, 0, &pl, H, W));
+    CKR(ensure_s3fd_detect(ctx, pl));
+    pl->pins++;
+    g->det_plans[k].plan = pl;
+    g->det_plans[k].epoch = ctx->plan_epoch[W2L_NET_S3FD];
+    *out = pl;
+    return W2L_OK;
+}
+
+// one S3FD launch over fr[0, n) (n <= B frames of one size) on the detection stream, its rects read back to pinned memory
+static int group_det_launch(w2l_stream_group* g, const std::pair<GroupSession*, long long>* fr, int n, int B) {
+    w2l_ctx* ctx = g->ctx;
+    const int H = fr[0].first->sched.d.H, W = fr[0].first->sched.d.W;
+    Plan* pl;
+    CKR(group_det_plan(g, H, W, B, &pl));
+    std::unique_ptr<DetJob> j;
+    if (!g->det_free.empty()) { j = std::move(g->det_free.back()); g->det_free.pop_back(); }
+    else {
+        j.reset(new DetJob());
+        CKR(j->dev.grow(ctx, kDetDevBytes));
+        CKR(j->host.alloc(kDetHostBytes));
+    }
+    const uint8_t** ptrs = (const uint8_t**)j->host.p;
+    const size_t frame_bytes = (size_t)H * W * 3;
+    for (int k = 0; k < B; ++k) {
+        const auto& f = fr[std::min(k, n - 1)];
+        ptrs[k] = f.first->frames + (size_t)f.second * frame_bytes;
+    }
+    for (int k = 0; k < n; ++k) { j->sid[k] = fr[k].first->id; j->frame[k] = (int32_t)fr[k].second; }
+    j->n = n;
+    uint8_t* dv = j->dev.p;
+    CK(cudaMemcpyAsync(dv + kDetDevPtrs, ptrs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, g->s_det));
+    const long long l0 = ctx->launches;
+    S3fdRun run{nullptr, 1, 1, (float*)(dv + kDetDevDets), (int32_t*)(dv + kDetDevCounts)};
+    run.frame_ptrs = (const uint8_t* const*)(dv + kDetDevPtrs);
+    CKR(run_plan(ctx, pl, nullptr, nullptr, nullptr, nullptr, g->s_det, false, nullptr, &run));
+    s3fd_rect_export_kernel<<<1, 32, 0, g->s_det>>>((const float*)(dv + kDetDevDets), (const int*)(dv + kDetDevCounts), n, 1,
+                                                    (int32_t*)(dv + kDetDevRects));
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync((uint8_t*)j->host.p + kDetHostRects, dv + kDetDevRects, (size_t)n * 5 * 4, cudaMemcpyDeviceToHost, g->s_det));
+    g->calls += 2 + (ctx->launches - l0);
+    g->det_busy.push_back(std::move(j));
+    return W2L_OK;
+}
+
+// Queue the detection of frames [det_launched, upto) of each (session, upto), pooled per frame size in launches of
+// det_bucket frames, then record ev_det.
+static int group_detect(w2l_stream_group* g, const std::vector<std::pair<GroupSession*, long long>>& upto) {
+    std::map<std::pair<int, int>, std::vector<std::pair<GroupSession*, long long>>> by_size;
+    for (const auto& u : upto) {
+        GroupSession* s = u.first;
+        for (long long f = s->det_launched; f < u.second; ++f) by_size[{s->sched.d.H, s->sched.d.W}].push_back({s, f});
+    }
+    if (by_size.empty()) return W2L_OK;
+    for (const auto& kv : by_size) {
+        const auto& fr = kv.second;
+        for (size_t i = 0; i < fr.size();) {
+            const int B = det_bucket((long long)(fr.size() - i));
+            const int n = (int)std::min<size_t>((size_t)B, fr.size() - i);
+            CKR(group_det_launch(g, fr.data() + i, n, B));
+            i += n;
+        }
+    }
+    for (const auto& u : upto) u.first->det_launched = std::max(u.first->det_launched, u.second);
+    CK(cudaEventRecord(g->ev_det, g->s_det));
+    g->calls++;
+    return W2L_OK;
+}
+
+// every busy job has completed (the caller waited): its rects go to their sessions, the job to the free list
+static void group_det_resolve(w2l_stream_group* g) {
+    for (auto& j : g->det_busy) {
+        const int32_t* o = (const int32_t*)((const uint8_t*)j->host.p + kDetHostRects);
+        for (int k = 0; k < j->n; ++k) {
+            auto f = g->sessions.find(j->sid[k]);
+            if (f == g->sessions.end()) continue;      // closed since
+            GroupSession* s = f->second.get();
+            s->det_status[j->frame[k]] = (int8_t)o[5 * k + 4];
+            if (o[5 * k + 4] == kRectFace) s->sched.set_rect(j->frame[k], o + 5 * k);
+        }
+        g->det_free.push_back(std::move(j));
+    }
+    g->det_busy.clear();
+}
+
+// The first frame below n whose detection failed: face_boxes' message (inference.py:91-93), or the non-finite box's.
+// Frames below n are read back by the time this is asked.
+static bool group_det_failed(GroupSession* s, long long n, std::string* msg) {
+    while (s->det_ok < n && s->det_status[s->det_ok] == kRectFace) ++s->det_ok;
+    if (s->det_ok >= n) return false;
+    const long long f = s->det_ok;
+    char buf[160];
+    if (s->det_status[f] == kRectNone)
+        snprintf(buf, sizeof(buf), "Face not detected in frame %lld! Ensure the video contains a face in all the frames.", f);
+    else if (s->det_status[f] == kRectNonFinite)
+        snprintf(buf, sizeof(buf), "Face detector returned a non-finite box in frame %lld", f);
+    else
+        snprintf(buf, sizeof(buf), "frame %lld: its detection was not read back", f);
+    *msg = buf;
+    return true;
+}
 
 static void group_release(w2l_stream_group* g, GroupBucket* b) {
     if (b->plan && b->epoch == g->ctx->plan_epoch[W2L_NET_GENERATOR]) b->plan->pins--;
@@ -201,7 +369,7 @@ static int group_step(w2l_stream_group* g, const GroupPend* pend, int n, cudaStr
 
 // what a tick does with one of its sessions
 struct GroupItem {
-    GroupSession* s = nullptr;       // null: skipped (the session failed on a NaN in an earlier tick)
+    GroupSession* s = nullptr;       // null: skipped (the session failed in an earlier tick)
     const float* pcm = nullptr;
     long long n = 0, done = 0;       // samples, and those already in the ring
     bool finish = false, device = false, failed = false;
@@ -335,12 +503,18 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
         ctx->launches++; g->calls++;
         CK(cudaGetLastError());
     }
+    // the detection launched so far is read back within the same wait
+    if (!g->det_busy.empty()) {
+        CK(cudaStreamWaitEvent(g->s_mel, g->ev_det, 0));
+        g->calls++;
+    }
     // every flag in one copy: the round's host wait (the upload's pinned buffer and host pcm are read by then)
     CK(cudaMemcpyAsync(g->nan_host.p, g->nan, (size_t)g->n_slots * 4, cudaMemcpyDeviceToHost, g->s_mel));
     CK(cudaEventRecord(g->ev_mel, g->s_mel));
     CK(cudaEventSynchronize(g->ev_mel));
     CK(cudaStreamWaitEvent(st, g->ev_mel, 0));
     g->calls += 3; g->waits++;
+    group_det_resolve(g);
 
     const int* flags = (const int*)g->nan_host.p;
     for (size_t i = 0; i < items.size(); ++i) {
@@ -352,16 +526,26 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
         s->mel.f_next = std::max(s->mel.f_next, p.f_end);
         it.done += p.piece;
         if (it.done < it.n || (it.finish && !p.fin)) *more = true;
-        if (flags[s->slot]) {     // its rows of this tick do not run
-            s->nan = true;
+        auto fail_session = [&](const std::string& msg) {   // its rows of this tick do not run
+            s->failed = true;
+            s->msg = msg;
             it.failed = true;
             status[i] = W2L_EINVAL;
             pend->erase(std::remove_if(pend->begin(), pend->end(), [s](const GroupPend& q) { return q.s == s; }), pend->end());
-            continue;
-        }
+        };
+        std::string msg;
+        if (flags[s->slot]) { fail_session(kMelNanMsg); continue; }
+        // a detected session fails at the tick whose rows first read a frame without a usable box
+        if (s->detect && group_det_failed(s, s->sched.need(it.last), &msg)) { fail_session(msg); continue; }
         StreamSched::At a;
         if (p.fin) a = it.last;
         else CKR(s->sched.at(s->mel.L, false, &a));
+        if (s->detect) {   // its rows need the rects read back above
+            bool bad = false;
+            for (long long r = it.first + it.queued; r < a.n_fixed && !bad; ++r)
+                if (s->sched.row(r, a, &it.rows[(size_t)(r - it.first) * W2L_STREAM_ROW]) != W2L_OK) bad = true;
+            if (bad) { fail_session(g_err); continue; }
+        }
         const size_t frame_bytes = (size_t)s->sched.d.H * s->sched.d.W * 3;
         for (long long r = it.first + it.queued; r < a.n_fixed; ++r, ++it.queued)
             pend->push_back(GroupPend{s, &it.rows[(size_t)(r - it.first) * W2L_STREAM_ROW],
@@ -392,7 +576,7 @@ static int group_tick(w2l_stream_group* g, int n, const int32_t* ids, const floa
         status[i] = W2L_OK;
         first_index[i] = s->emitted;
         n_out[i] = 0;
-        if (s->nan) { status[i] = W2L_EINVAL; continue; }
+        if (s->failed) { status[i] = W2L_EINVAL; continue; }
         if (s->finished) return fail(W2L_ESTATE, "session %d is finished", ids[i]);
         const long long ns = n_samples[i];
         const float* p = pcm ? pcm[i] : nullptr;
@@ -411,9 +595,15 @@ static int group_tick(w2l_stream_group* g, int n, const int32_t* ids, const floa
         it.out = out[i];
         it.first = s->emitted;
         it.rows.resize((size_t)need * W2L_STREAM_ROW);
-        for (long long r = 0; r < need; ++r) CKR(s->sched.row(it.first + r, it.last, &it.rows[(size_t)r * W2L_STREAM_ROW]));
+        if (!s->detect)   // a detected session's rows are made once its rects are read back (group_round)
+            for (long long r = 0; r < need; ++r) CKR(s->sched.row(it.first + r, it.last, &it.rows[(size_t)r * W2L_STREAM_ROW]));
         it.s = s;
     }
+    // ---- detection of the frames this tick's rows read that no launch covers yet ----
+    std::vector<std::pair<GroupSession*, long long>> upto;
+    for (const GroupItem& it : items)
+        if (it.s && it.s->detect) upto.push_back({it.s, it.s->sched.need(it.last)});
+    CKR(group_detect(g, upto));
     // ---- rounds (one unless a piece exceeds what a session's rings take), then the partial last step ----
     std::vector<GroupPend> pend;
     bool more = true;
@@ -421,7 +611,16 @@ static int group_tick(w2l_stream_group* g, int n, const int32_t* ids, const floa
     if (!pend.empty()) CKR(group_step(g, pend.data(), (int)pend.size(), st));
     for (int i = 0; i < n; ++i)
         if (items[i].s && !items[i].failed) n_out[i] = items[i].s->emitted - items[i].first;
-    return W2L_OK;
+    // ---- prefetch: the frames 200 ms more audio would need, read back by a later tick's wait ----
+    upto.clear();
+    for (const GroupItem& it : items) {
+        GroupSession* s = it.s;
+        if (!s || !s->detect || s->failed || s->finished) continue;
+        StreamSched::At a;
+        CKR(s->sched.at(s->mel.L + kDetAheadSamples, false, &a));
+        upto.push_back({s, s->sched.need(a)});
+    }
+    return group_detect(g, upto);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -453,6 +652,9 @@ int w2l_stream_group_create(w2l_ctx* ctx, int max_batch, int audio_ring_log2, w2
     CKR(g->cap.create());
     CKR(g->ev_mel.create());
     CKR(g->ev_caller.create());
+    CKR(g->s_det.create());
+    CKR(g->ev_det.create());
+    CKR(g->ev_open.create());
     for (Event& e : g->table_done) CKR(e.create());
     for (Event& e : g->step_done) CKR(e.create());
     CKR(g->table.grow(ctx, (size_t)max_batch * sizeof(GroupRow)));
@@ -465,13 +667,13 @@ int w2l_stream_group_create(w2l_ctx* ctx, int max_batch, int audio_ring_log2, w2
     return W2L_OK;
 }
 
-int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
-                          const int32_t* rects_host, int32_t* session_id) {
+static int group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d, const int32_t* rects_host,
+                      bool detect, int32_t* session_id) {
     if (!g || !frames_dev || !d || !session_id) return fail(W2L_EINVAL, "null argument");
     w2l_ctx* ctx = g->ctx;
     DeviceGuard dg(ctx->device);
     std::unique_ptr<GroupSession> s(new GroupSession());
-    CKR(s->sched.init(d, rects_host));
+    CKR(s->sched.init(d, rects_host, detect));
     if ((long long)d->H * d->W * 3 > INT32_MAX) return fail(W2L_EINVAL, "a %dx%d frame: need fewer than 2^31 bytes", d->H, d->W);
     cudaPointerAttributes pa;
     const cudaError_t e = cudaPointerGetAttributes(&pa, frames_dev);
@@ -479,6 +681,12 @@ int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const 
     if (pa.type != cudaMemoryTypeDevice || pa.device != ctx->device)
         return fail(W2L_EINVAL, "frames must be device memory of the context's device %d", ctx->device);
     if (!ctx->nets[W2L_NET_GENERATOR].loaded) return fail(W2L_ESTATE, "generator weights not loaded");
+    if (detect) {
+        if (!ctx->nets[W2L_NET_S3FD].loaded) return fail(W2L_ESTATE, "S3FD weights not loaded");
+        if (d->H < 32 || d->W < 32) return fail(W2L_EINVAL, "S3FD needs frames of at least 32 x 32, got %dx%d", d->H, d->W);
+        s->detect = true;
+        s->det_status.assign((size_t)d->F, (int8_t)-1);
+    }
     s->frames = frames_dev;
     // as the session's: the frames of every row not yet run (< max_batch + 4 chunks) beside a whole audio ring of new ones
     const long long ra = 1LL << g->ring_log2;
@@ -490,8 +698,31 @@ int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const 
     s->slot = slot;
     s->id = g->next_id++;
     *session_id = s->id;
+    if (detect) {
+        // The frames the first 400 ms of audio need, launched without waiting.  They were written by work the caller
+        // queued before this call on the legacy default stream (or completed).
+        StreamSched::At a;
+        int r = s->sched.at(kDetOpenSamples, false, &a);
+        if (r == W2L_OK && cudaEventRecord(g->ev_open, cudaStreamLegacy) == cudaSuccess &&
+            cudaStreamWaitEvent(g->s_det, g->ev_open, 0) == cudaSuccess)
+            r = group_detect(g, {{s.get(), s->sched.need(a)}});
+        else if (r == W2L_OK)
+            r = fail(W2L_ECUDA, "%s", cudaGetErrorString(cudaGetLastError()));
+        if (r != W2L_OK) { g->free_slots.push_back(slot); return r; }   // launches already queued find no session
+        g->det_sizes[{d->H, d->W}]++;
+    }
     g->sessions[s->id] = std::move(s);
     return W2L_OK;
+}
+
+int w2l_stream_group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
+                          const int32_t* rects_host, int32_t* session_id) {
+    return group_open(g, frames_dev, d, rects_host, false, session_id);
+}
+
+int w2l_stream_group_open_detect(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_stream_desc* d,
+                                 int32_t* session_id) {
+    return group_open(g, frames_dev, d, nullptr, true, session_id);
 }
 
 int w2l_stream_group_close(w2l_stream_group* g, int32_t session_id) {
@@ -501,7 +732,15 @@ int w2l_stream_group_close(w2l_stream_group* g, int32_t session_id) {
     DeviceGuard dg(g->ctx->device);
     CK(cudaDeviceSynchronize());   // queued steps may still read the session's rings
     g->free_slots.push_back(f->second->slot);
+    if (f->second->detect) {
+        const std::pair<int, int> hw(f->second->sched.d.H, f->second->sched.d.W);
+        if (--g->det_sizes[hw] == 0) {   // the last detecting session of its size: unpin that size's plans
+            g->det_sizes.erase(hw);
+            group_det_release(g, hw.first, hw.second);
+        }
+    }
     g->sessions.erase(f);
+    group_det_resolve(g);          // every launch is complete: its buffers are free again
     return W2L_OK;
 }
 
@@ -513,7 +752,7 @@ int w2l_stream_group_pending(const w2l_stream_group* g, int n, const int32_t* id
         if (f == g->sessions.end()) return fail(W2L_EINVAL, "session %d is not open in this group", ids[i]);
         const GroupSession* s = f->second.get();
         n_out[i] = 0;
-        if (s->nan || s->finished) continue;
+        if (s->failed || s->finished) continue;
         if (n_samples[i] < 0) return fail(W2L_EINVAL, "session %d: bad audio piece (%lld samples)", ids[i], (long long)n_samples[i]);
         StreamSched::At a;
         CKR(s->sched.at(s->mel.L + n_samples[i], finish && finish[i] != 0, &a));
@@ -531,7 +770,7 @@ int w2l_stream_group_tick(w2l_stream_group* g, int n, const int32_t* ids, const 
 const char* w2l_stream_group_error(const w2l_stream_group* g, int32_t session_id) {
     if (!g) return "";
     auto f = g->sessions.find(session_id);
-    return f != g->sessions.end() && f->second->nan ? kMelNanMsg : "";
+    return f != g->sessions.end() && f->second->failed ? f->second->msg.c_str() : "";
 }
 
 int w2l_stream_group_counters(const w2l_stream_group* g, int64_t* calls, int64_t* host_waits, int64_t* steps) {
@@ -547,6 +786,8 @@ int w2l_stream_group_destroy(w2l_stream_group* g) {
     DeviceGuard dg(g->ctx->device);
     cudaDeviceSynchronize();   // queued steps may still read the group's buffers
     for (auto& b : g->buckets) group_release(g, b.get());
+    for (const DetPlan& p : g->det_plans)
+        if (p.plan && p.epoch == g->ctx->plan_epoch[W2L_NET_S3FD]) p.plan->pins--;
     delete g;
     return W2L_OK;
 }

@@ -21,16 +21,20 @@ struct S3fdIngestParams {
     uint16_t* dst;             // [N][H][Wp][Cpix], image column x at column x + x_off (zero borders pre-set)
     int N, H, W, Cpad, Wp, x_off, Cpix, lo_off;
     int reverse;
+    const unsigned char* const* srcs;   // kGather: image n is the (H, W, 3) frame srcs[n]; src unused
 };
 
-template <bool kBF16>
+// kGather: each image through the frame-pointer table, so one launch takes frames of several videos of one size
+template <bool kBF16, bool kGather = false>
 __global__ void s3fd_ingest_u8_kernel(const S3fdIngestParams p) {
     const long long total = (long long)p.N * p.H * p.W;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int x = (int)(i % p.W);
         const int y = (int)((i / p.W) % p.H);
         const int n = (int)(i / ((long long)p.W * p.H));
-        const unsigned char* s = p.src + i * 3;
+        const unsigned char* s;
+        if constexpr (kGather) s = p.srcs[n] + (i - (long long)n * p.W * p.H) * 3;
+        else s = p.src + i * 3;
         const int m[3] = {104, 117, 123};
         uint16_t h[4];
 #pragma unroll
@@ -232,6 +236,27 @@ __global__ void __launch_bounds__(kNmsThreads) s3fd_nms_kernel(const S3fdDetPara
         p.counts[b] = kept;
         p.path[b] = fast ? 0 : 1;
     }
+}
+
+// ---- (d) rect export -----------------------------------------------------------------------------------------------------
+// get_detections_for_batch_u8's result for image b < n (api.py: the first box, np.clip(d[:4], 0, None), int() of each):
+// out[b] = (x1, y1, x2, y2, status).  Finiteness is tested before the clip, because fmaxf(NaN, 0) is 0 while np.clip
+// keeps the NaN and int() then raises.  Coordinates are clamped to 2^30 before the truncating conversion, so that the
+// padding arithmetic after it cannot overflow int32.
+constexpr int kRectFace = 0, kRectNone = 1, kRectNonFinite = 2;
+
+__global__ void s3fd_rect_export_kernel(const float* dets, const int* counts, int n, int max_det, int32_t* out) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    int32_t* o = out + (size_t)b * 5;
+    const float* d = dets + (size_t)b * max_det * 5;
+    int status = counts[b] > 0 ? kRectFace : kRectNone;
+    for (int k = 0; k < 4; ++k) {
+        const float v = status == kRectNone ? 0.0f : d[k];
+        if (!isfinite(v)) status = kRectNonFinite;
+        o[k] = isfinite(v) ? (int32_t)fminf(fmaxf(v, 0.0f), 1073741824.0f) : 0;
+    }
+    o[4] = status;
 }
 
 }  // namespace w2l

@@ -83,23 +83,27 @@ class NativeNet(nn.Module):
             self._w2l_key = None
         key = self._weights_key()
         if key != self._w2l_key:
-            tensors, keep = {}, []
-            for name, t in self.state_dict(keep_vars=True).items():
-                if not t.dtype.is_floating_point:
-                    continue
-                if not t.is_cuda:
-                    raise _lib.W2LError(f"parameter {name} is on {t.device}; move the module with .to('cuda') first")
-                tc = t.detach().contiguous().float()
-                keep.append(tc)
-                tensors[name] = (tc.data_ptr(), tc.numel())
             stream = torch.cuda.current_stream(ref.device).cuda_stream
-            self._w2l_ctx.load_weights(self.NET, tensors, stream)
+            self._load_into(self._w2l_ctx, stream)
             self._w2l_key = key
             self._w2l_range_checked = False
             if self.precision != _lib.PREC_BF16:
                 # the flag is one per DEVICE (any context's kernels set it): start this model's check window clean
                 self._w2l_ctx.f16_overflow(clear=True, stream=stream)
         return self._w2l_ctx
+
+    def _load_into(self, ctx, stream):
+        """Hand the current parameters to `ctx` (w2l_load_weights of this network)."""
+        tensors, keep = {}, []
+        for name, t in self.state_dict(keep_vars=True).items():
+            if not t.dtype.is_floating_point:
+                continue
+            if not t.is_cuda:
+                raise _lib.W2LError(f"parameter {name} is on {t.device}; move the module with .to('cuda') first")
+            tc = t.detach().contiguous().float()
+            keep.append(tc)
+            tensors[name] = (tc.data_ptr(), tc.numel())
+        ctx.load_weights(self.NET, tensors, stream)
 
     def _wants_grad(self) -> bool:
         return any(p.requires_grad for p in self.parameters())

@@ -12,7 +12,8 @@ include/w2l.h `w2l_stream_*`.
 Two behavioural differences, both in when an error is raised: inference.py raises on a NaN mel before it produces
 anything, the session raises the same ValueError from the push that computes the NaN frame (and from every later call),
 and frames returned by earlier pushes stay valid; and rects with a None (no face) raise when the session is created,
-even for frames past the ones a short utterance reaches, which inference.py would not look at.
+even for frames past the ones a short utterance reaches, which inference.py would not look at.  `LipSyncServer` with a
+detector finds the faces itself and removes the second difference for the sessions it detects.
 """
 import ctypes as C
 
@@ -199,9 +200,17 @@ class LipSyncServer:
     returns the `ValueError` (the reference's message) as that session's value instead of raising, the other sessions'
     frames are returned as usual, and every later tick that names the failed session raises that `ValueError` before
     anything runs.  A bad argument raises before anything runs, for the whole tick.  `audio_ring_log2` sets the audio
-    ring of every session (0: 2^16 samples)."""
+    ring of every session (0: 2^16 samples).
 
-    def __init__(self, model, max_batch=128, audio_ring_log2=0):
+    detector: a `face_detection.FaceAlignment` (as inference.py:69-70 builds it) of the model's precision.  With it,
+    `open(frames, fps)` without rects or box finds each frame's face as `get_detections_for_batch_u8` does on
+    inference.py's BGR frames, on the device and only for the frames the session's audio reaches, just before a tick
+    needs them (DESIGN.md section 3.10); pads and nosmooth apply as with rects.  Its S3FD weights are loaded into the
+    model's context and reloaded when they change (rects already found are kept).  A frame that a tick needs without a
+    face fails that session as a NaN does, with face_boxes' message naming the frame; a frame the utterance never
+    reaches fails nothing."""
+
+    def __init__(self, model, max_batch=128, audio_ring_log2=0, detector=None):
         if isinstance(max_batch, bool) or int(max_batch) != max_batch or int(max_batch) < 1:
             raise ValueError(f"max_batch must be a positive integer, got {max_batch!r}")
         self.model = model
@@ -211,6 +220,18 @@ class LipSyncServer:
         self._ctx = None
         self._sessions = {}   # id -> (frames, (H, W))
         self._failed = {}     # id -> message
+        self.detector = detector
+        self._det_loaded = None   # (context, weights key) of the S3FD weights in the model's context
+        if detector is not None:
+            self._s3fd()
+
+    def _s3fd(self):
+        """The detector's S3FD module, checked against the model's precision."""
+        net = self.detector.face_detector.face_detector
+        if net.precision != self.model.precision:
+            raise ValueError(f"the detector's precision ({net.precision}) differs from the model's "
+                             f"({self.model.precision}): detection inside the server runs in the model's context")
+        return net
 
     def _group(self, frames):
         ctx = self.model._ensure(frames)   # reloads the weights if the model's parameters changed
@@ -220,6 +241,12 @@ class LipSyncServer:
             self._h, self._ctx, self._lib = h, ctx, ctx.lib
         elif ctx is not self._ctx:
             raise L.W2LError("the model moved to another device or context since the server was created")
+        if self.detector is not None:   # the detector's weights, into the model's context, reloaded when they change
+            net = self._s3fd()
+            key = (ctx, net._weights_key())
+            if self._det_loaded is None or self._det_loaded[0] is not key[0] or self._det_loaded[1] != key[1]:
+                net._load_into(ctx, torch.cuda.current_stream(frames.device).cuda_stream)
+                self._det_loaded = key
         return ctx
 
     def open(self, frames_u8, fps, rects=None, pads=(0, 10, 0, 0), nosmooth=False, box=None):
@@ -230,17 +257,28 @@ class LipSyncServer:
             raise ValueError(f"expected uint8 (F,H,W,3) frames, got {frames_u8.dtype} {tuple(frames_u8.shape)}")
         if not (float(fps) > 0) or not np.isfinite(float(fps)):
             raise ValueError(f"fps must be positive and finite, got {fps!r}")
-        if rects is None and box is None:
+        detect = rects is None and box is None
+        if detect and self.detector is None:
             raise ValueError("pass the detector rects of every frame or one fixed box")
         F, H, W = (int(v) for v in frames_u8.shape[:3])
         desc = _desc(F, H, W, fps, pads, nosmooth, box)
-        ra = _rects_array(rects, F) if box is None else None
+        ra = _rects_array(rects, F) if box is None and not detect else None
         frames = frames_u8.contiguous()
         ctx = self._group(frames)
         self.model._same_device(ctx, frames)
         sid = C.c_int32()
-        _raise(self._lib.w2l_stream_group_open(self._h, C.c_void_p(frames.data_ptr()), C.byref(desc),
-                                               ra.ctypes.data_as(C.c_void_p) if ra is not None else None, C.byref(sid)))
+        if detect:
+            # the native side orders its first detection after the legacy default stream; frames written on another
+            # stream must be complete
+            cur = torch.cuda.current_stream(frames.device)
+            if cur.cuda_stream != 0:
+                cur.synchronize()
+            _raise(self._lib.w2l_stream_group_open_detect(self._h, C.c_void_p(frames.data_ptr()), C.byref(desc),
+                                                          C.byref(sid)))
+        else:
+            _raise(self._lib.w2l_stream_group_open(self._h, C.c_void_p(frames.data_ptr()), C.byref(desc),
+                                                   ra.ctypes.data_as(C.c_void_p) if ra is not None else None,
+                                                   C.byref(sid)))
         self._sessions[sid.value] = (frames, (H, W))
         return sid.value
 
@@ -332,6 +370,15 @@ class LipSyncServer:
             self.close()
         except Exception:
             pass
+
+
+def detect_need(n_samples, F, H, W, fps, pads=(0, 10, 0, 0), nosmooth=False, final=False):
+    """Host only (no GPU): the frames [0, need) whose rects the rows that `n_samples` fix read, as
+    `w2l_stream_detect_need` computes them for a detecting session."""
+    n = C.c_int64()
+    d = _desc(F, H, W, fps, pads, nosmooth, None)
+    _raise(L.get_lib().w2l_stream_detect_need(C.byref(d), int(n_samples), 1 if final else 0, C.byref(n)))
+    return n.value
 
 
 def stream_buckets(max_batch, n_rows):
