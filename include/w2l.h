@@ -326,8 +326,10 @@ int w2l_stream_schedule(const w2l_stream_desc* d, const int32_t* rects_host, int
 int w2l_stream_detect_need(const w2l_stream_desc* d, int64_t n_samples, int final_, int64_t* n_frames);
 
 /* Every step runs the generator at exactly `batch` rows (one plan; rows past the ready ones repeat the last ready row
- * and are dropped), from a CUDA graph captured once per session and replayed (W2L_DISABLE_STREAMGRAPH=1 launches the
- * same kernels directly).  The generator weights must be loaded; loading new ones between pushes is allowed.
+ * and are not pasted): gather, crop, generator and paste into out_dev, from a CUDA graph captured once per session and
+ * replayed (W2L_DISABLE_STREAMGRAPH=1 launches the same kernels directly).  frames_dev is device memory on the
+ * context's device, with frames of fewer than 2^31 bytes (H * W * 3).  The generator weights must be loaded; loading
+ * new ones between pushes is allowed.
  * _push / _finish write n_out output frames (n_out, H, W, 3) uint8 to out_dev; they are output indices
  * first_index .. first_index + n_out - 1.  Size out_dev with w2l_stream_pending.  A push whose audio gives a mel frame
  * holding a NaN fails with W2L_EINVAL and the reference's message (inference.py:228-229) and writes no frame of a

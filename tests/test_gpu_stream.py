@@ -279,7 +279,9 @@ def test_pinned_plan_survives_lru_eviction(gen):
 
 
 def test_bad_arguments(gen):
-    from wav2lip_b200 import _lib
+    import ctypes as C
+
+    from wav2lip_b200 import _lib, stream
     from wav2lip_b200.stream import LipSyncSession
     frames, rects = _video(6, seed=11)
     launches = gen._w2l_ctx.launch_count() if gen._w2l_ctx else None
@@ -293,5 +295,11 @@ def test_bad_arguments(gen):
         LipSyncSession(gen, frames, 0.0, rects=rects)
     with pytest.raises(ValueError):
         LipSyncSession(gen, frames, 25.0)
+    # a frame of 2^31 bytes or more (the paste's offsets within a frame are 32-bit), described over a small real video
+    ctx = gen._ensure(frames)
+    big = stream._desc(1, 1, 2 ** 31 // 3 + 1, 25.0, (0, 10, 0, 0), False, (0, 1, 0, 1))
+    h = C.c_void_p()
+    with pytest.raises(_lib.W2LError, match=r"2\^31"):
+        _lib.check(ctx.lib.w2l_stream_create(ctx.h, C.c_void_p(frames.data_ptr()), C.byref(big), None, 1, C.byref(h)))
     if launches is not None:
         assert gen._w2l_ctx.launch_count() == launches

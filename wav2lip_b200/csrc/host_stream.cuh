@@ -1,6 +1,8 @@
 // host_stream.cuh — streaming: the mel rings behind w2l_melstream_* and the lip-sync session behind w2l_stream_*
 // (DESIGN.md section 3.8).  The scheduling rules (which rows the audio received so far fixes) are host code with no
-// device state, exported as w2l_stream_schedule so that they can be tested without a GPU.
+// device state, exported as w2l_stream_schedule so that they can be tested without a GPU.  The piece planner
+// (MelRing::plan), the generator steps (StepRunner) and the ring-reader tracking (RingReaders) serve stream groups
+// (host_stream_group.cuh) as well.
 // Part of the single translation unit w2l_api.cu (included there, after the plans).
 #pragma once
 
@@ -50,6 +52,17 @@ static int pcm_kind(const w2l_ctx* ctx, const float* p, int* kind) {
 // ------------------------------------------------------------------------------------------------
 // mel rings: audio by absolute sample index, mel by absolute frame index, both power-of-two long
 // ------------------------------------------------------------------------------------------------
+// The next piece of a stream's input and what it makes final (MelRing::plan).
+struct MelPiece {
+    long long n = 0;            // input samples
+    ResampleClock clk;          // the resampling clock after them
+    long long L = 0;            // the 16 kHz length after them
+    bool input_end = false;     // the end of the input is resampled with them (its right wings stop there)
+    long long f_end = 0;        // mel frames final after them
+    long long L_end = -1;       // at finish: the final length, where the last frames reflect; else -1
+    bool fin = false;           // the piece ends the stream: frames [f_next, f_end) are all there are
+};
+
 struct MelRing {
     w2l_ctx* ctx = nullptr;
     long long ra = 0, rm = 0;   // audio ring (samples), mel ring (frames)
@@ -68,7 +81,6 @@ struct MelRing {
     long long rsrc = 0;         // input ring length (samples)
     DevMem<float> src;
     DevMem<double> reg0;        // block start registers of one launch
-    std::vector<double> starts;
     const double2* wd = nullptr;
 
     bool resampling() const { return sr != 16000; }
@@ -106,45 +118,6 @@ struct MelRing {
         return std::min(by_src, by_out);
     }
 
-    // The outputs n_in samples make final (finish: all of them, the right wing stopping at the end) into the audio ring;
-    // at most max_out of them (what max_piece allows), or nothing is done and W2L_ESTATE returned.
-    int resample(bool finish, long long max_out, cudaStream_t st) {
-        ResampleClock c = clk;
-        if (c.advance(n_in, finish, nullptr) - clk.t > max_out)
-            return fail(W2L_ESTATE, "audio ring too small for the resampled piece");
-        starts.clear();
-        const long long t0 = clk.t;
-        const long long t1 = clk.advance(n_in, finish, &starts);
-        if (t1 == t0) return W2L_OK;
-        CK(cudaMemcpyAsync(reg0.p, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
-        const ResampleParams p = resample_params(clk, wd, reg0, t0, t1, finish ? clk.n_res(n_in) : (1LL << 62));
-        ResampleRingParams r;
-        r.src = src; r.src_mask = rsrc - 1; r.n_in = finish ? n_in : (1LL << 62);
-        r.audio = audio; r.audio_mask = ra - 1; r.nan = nan;
-        resample_ring_kernel<<<(unsigned)starts.size(), RS_THREADS, 0, st>>>(p, r);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        L = t1;
-        return W2L_OK;
-    }
-
-    // a piece of input (see append), resampled when the stream has an input rate; n <= max_input(max_out)
-    int feed(const float* pcm, long long n, long long max_out, cudaStream_t st) {
-        if (!resampling()) return append(pcm, n, st);
-        long long done = 0;
-        while (done < n) {
-            const long long at = (n_in + done) & (rsrc - 1);
-            const long long k = std::min(n - done, rsrc - at);
-            CK(cudaMemcpyAsync(src.p + at, pcm + done, (size_t)k * 4, cudaMemcpyDefault, st));
-            done += k;
-        }
-        n_in += n;
-        return resample(false, max_out, st);
-    }
-
-    // at finish: the outputs that reach the end of the input (at most max_out: see max_piece)
-    int end_input(long long max_out, cudaStream_t st) { return resampling() ? resample(true, max_out, st) : W2L_OK; }
-
     int init(w2l_ctx* c, int audio_log2, long long min_mel_frames) {
         ctx = c;
         if (audio_log2 == 0) audio_log2 = 16;
@@ -169,32 +142,97 @@ struct MelRing {
         return std::min(by_audio, by_mel);
     }
 
-    // pcm: host (any kind) or device memory; copied into the ring at absolute positions [L, L + n)
-    int append(const float* pcm, long long n, cudaStream_t st) {
-        long long done = 0;
-        while (done < n) {
-            const long long at = (L + done) & (ra - 1);
-            const long long k = std::min(n - done, ra - at);
-            CK(cudaMemcpyAsync(audio.p + at, pcm + done, (size_t)k * 4, cudaMemcpyDefault, st));
-            done += k;
+    // The next piece: at most `left` input samples (ends: the input ends after them), as many as overwrite nothing that
+    // is still read (max_piece, max_input; keep: the oldest mel frame the consumer still needs).  starts gets the
+    // register of every RS_THREADS-th output the piece resamples.  The end of the input is taken only once its last
+    // outputs fit the audio ring and its last frames, from the right-aligned last chunk (M - 16) on, fit the mel ring;
+    // until then the piece stops short of it and a later one, after the consumer has moved on, ends the stream.  A piece
+    // that would make no progress is W2L_ESTATE.
+    int plan(long long left, bool ends, long long keep, MelPiece* out, std::vector<double>* starts) const {
+        const long long room = max_piece(keep);
+        MelPiece p;
+        p.n = std::max(0LL, std::min(left, max_input(room)));
+        p.input_end = ends && p.n == left;
+        p.L = L + p.n;
+        starts->clear();
+        if (resampling()) {
+            p.clk = clk;
+            p.L = p.clk.advance(n_in + p.n, p.input_end, starts);
+            if (p.input_end && p.L - L > room) {
+                starts->clear();
+                p.clk = clk;
+                p.L = p.clk.advance(n_in + p.n, false, starts);
+                p.input_end = false;
+            }
         }
-        L += n;
+        p.f_end = mel_final_frames(p.L);
+        if (p.input_end) {
+            const long long M = 1 + p.L / MEL_HOP;   // the mel frames of the whole input (StreamSched::at at final)
+            if (M - std::min(keep, M - 16) <= rm) { p.fin = true; p.f_end = M; p.L_end = p.L; }
+        }
+        if (p.n == 0 && p.L == L && !p.fin) return fail(W2L_ESTATE, "audio or mel ring too small for the next piece");
+        *out = p;
         return W2L_OK;
     }
 
-    // frames [f_next, f_end); L_end >= 0 only at finish (reflection at the end of the utterance)
-    int compute(const MelParams& tables, long long f_end, long long L_end, cudaStream_t st) {
-        if (f_end <= f_next) return W2L_OK;
+    // where a piece's input goes: the input ring of a resampling stream, else the audio ring
+    GroupScatter input_of(const MelPiece& p, const float* pcm) const {
+        if (resampling()) return GroupScatter{pcm, src.p, rsrc - 1, n_in, p.n};
+        return GroupScatter{pcm, audio.p, ra - 1, L, p.n};
+    }
+
+    void resample_args(const MelPiece& p, const double* reg, int* flag, ResampleParams* rp, ResampleRingParams* r) const {
+        const long long n1 = n_in + p.n;
+        *rp = resample_params(clk, wd, reg, L, p.L, p.input_end ? clk.n_res(n1) : (1LL << 62));
+        r->src = src; r->src_mask = rsrc - 1; r->n_in = p.input_end ? n1 : (1LL << 62);
+        r->audio = audio; r->audio_mask = ra - 1; r->nan = flag;
+    }
+
+    // the piece's frames [f_next, p.f_end); L_end >= 0 only at finish (reflection at the end of the utterance)
+    MelRingParams mel_args(const MelPiece& p, int* flag) const {
         MelRingParams r;
         r.audio = audio; r.audio_mask = ra - 1; r.mel = mel; r.mel_pitch = rm;
-        r.L = L_end >= 0 ? L_end : (1LL << 62);
-        r.f0 = f_next; r.f1 = f_end; r.nan = nan;
-        const long long blocks = (f_end - f_next + MEL_FPB - 1) / MEL_FPB;
-        mel_ring_kernel<<<(unsigned)blocks, MEL_THREADS, kMelSmemBytes, st>>>(tables, r);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        f_next = f_end;
+        r.L = p.L_end >= 0 ? p.L_end : (1LL << 62);
+        r.f0 = f_next; r.f1 = p.f_end; r.nan = flag;
+        return r;
+    }
+
+    // Queues a planned piece on st: its input (pcm: host memory of any kind, or device memory) copied into its ring at
+    // absolute positions, the outputs it makes final resampled into the audio ring, and, once `readers` (if any) has
+    // completed, its mel frames.  The ring is unchanged until commit.
+    int launch(const MelPiece& p, const float* pcm, const std::vector<double>& starts, const MelParams& tables,
+               cudaEvent_t readers, cudaStream_t st) {
+        const GroupScatter in = input_of(p, pcm);
+        for (long long done = 0; done < in.n;) {
+            const long long at = (in.at + done) & in.mask;
+            const long long k = std::min(in.n - done, in.mask + 1 - at);
+            CK(cudaMemcpyAsync(in.ring + at, pcm + done, (size_t)k * 4, cudaMemcpyDefault, st));
+            done += k;
+        }
+        if (!starts.empty()) {
+            CK(cudaMemcpyAsync(reg0.p, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
+            ResampleParams rp;
+            ResampleRingParams r;
+            resample_args(p, reg0, nan, &rp, &r);
+            resample_ring_kernel<<<(unsigned)starts.size(), RS_THREADS, 0, st>>>(rp, r);
+            ctx->launches++;
+            CK(cudaGetLastError());
+        }
+        if (p.f_end > f_next) {
+            if (readers) CK(cudaStreamWaitEvent(st, readers, 0));
+            const long long blocks = (p.f_end - f_next + MEL_FPB - 1) / MEL_FPB;
+            mel_ring_kernel<<<(unsigned)blocks, MEL_THREADS, kMelSmemBytes, st>>>(tables, mel_args(p, nan));
+            ctx->launches++;
+            CK(cudaGetLastError());
+        }
         return W2L_OK;
+    }
+
+    void commit(const MelPiece& p) {
+        if (resampling()) { clk = p.clk; n_in += p.n; }
+        L = p.L;
+        f_next = std::max(f_next, p.f_end);
+        finished = p.fin;
     }
 
     // the sticky NaN flag (waits for the work queued on st)
@@ -373,148 +411,222 @@ struct StreamSched {
 };
 
 // ------------------------------------------------------------------------------------------------
+// generator steps over stream rows: the lone session's and the stream group's (host_stream_group.cuh)
+// ------------------------------------------------------------------------------------------------
+constexpr int kStepSlots = 4;     // pinned staging slots of the per-step table in flight
+constexpr int kStepEvents = 16;   // step-completion events the ring-safety wait chooses from
+constexpr int kReaderTrack = 4;   // the last steps each session remembers (step id, lowest chunk start)
+
+// One step size: its generator plan and the CUDA graph of its step.  The plan is pinned against LRU eviction while held
+// and valid while epoch matches: it is erased, with every generator plan, only by drop_plans (new weights), which
+// bumps the epoch.  So a matching epoch means the plan, and every buffer the graph bakes, is alive and current.
+struct StepBucket {
+    int B = 0;
+    Plan* plan = nullptr;
+    uint64_t epoch = 0;
+    GraphExec exec;
+    bool warm = false;               // one uncaptured step ran on the current plan (kernel attributes are set)
+};
+
+// The step buffers.  Every pointer a step reads or writes is in its device table, one GroupRow per row, so the whole
+// step (gather, crop, generator, paste) is captured once per bucket and replayed whatever rows it runs.  The table
+// (max_batch rows) is shared by the buckets because steps run in order on the caller's stream; each step fills it with
+// one copy from a pinned slot.
+struct StepRunner {
+    w2l_ctx* ctx = nullptr;
+    int max_batch = 0;
+    DevMem<GroupRow> table;
+    PinnedMem table_host;            // kStepSlots x max_batch rows
+    Event table_done[kStepSlots];
+    Event step_done[kStepEvents];    // after step k (k % kStepEvents) on the caller's stream
+    long long count = 0;             // steps queued
+    DevMem<float> chunks;
+    DevMem<uint8_t> crops, preds;
+    Stream cap;                      // capture stream (the graph is launched on the caller's stream)
+    int64_t calls = 0, waits = 0;    // CUDA API submissions (launches, graph launches, copies, event records and waits)
+                                     // and host synchronisations (a stream group counts its ticks' here)
+
+    int init(w2l_ctx* c, int max_b) {
+        ctx = c;
+        max_batch = max_b;
+        for (Event& e : table_done) CKR(e.create());
+        for (Event& e : step_done) CKR(e.create());
+        CKR(table.grow(ctx, (size_t)max_batch * sizeof(GroupRow)));
+        CKR(table_host.alloc((size_t)kStepSlots * max_batch * sizeof(GroupRow)));
+        CKR(chunks.grow(ctx, (size_t)max_batch * 1280 * 4));
+        CKR(crops.grow(ctx, (size_t)max_batch * 96 * 96 * 3));
+        CKR(preds.grow(ctx, (size_t)max_batch * 96 * 96 * 3));
+        return cap.create();
+    }
+
+    void release(StepBucket* b) {
+        if (b->plan && b->epoch == ctx->plan_epoch[W2L_NET_GENERATOR]) b->plan->pins--;
+        b->plan = nullptr;
+        b->exec.reset();
+        b->warm = false;
+    }
+
+    int acquire(StepBucket* b) {
+        if (b->plan && b->epoch == ctx->plan_epoch[W2L_NET_GENERATOR]) return W2L_OK;
+        release(b);
+        Plan* pl;
+        CKR(get_plan(ctx, W2L_NET_GENERATOR, b->B, 0, &pl));
+        pl->pins++;
+        b->plan = pl;
+        b->epoch = ctx->plan_epoch[W2L_NET_GENERATOR];
+        return W2L_OK;
+    }
+
+    // gather + crop + generator + paste of B table rows
+    int body(const StepBucket& b, cudaStream_t st) {
+        const int B = b.B;
+        group_gather_kernel<<<(B * 1280 + 255) / 256, 256, 0, st>>>(table, B, chunks);
+        const long long total = (long long)B * 96 * 96;
+        group_crop_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16), 256, 0, st>>>(table, B, 96, crops);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+        CKR(run_plan(ctx, b.plan, chunks, crops, preds, nullptr, st, true));
+        // about 8 blocks per SM over the step, each row's frame split across gridDim.x of them
+        const dim3 grid((unsigned)std::max(1, (ctx->num_sms * 8 + B - 1) / B), (unsigned)B);
+        group_paste_kernel<<<grid, 256, 0, st>>>(preds, 96, table);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        return W2L_OK;
+    }
+
+    int capture(StepBucket* b) {
+        cudaGraph_t gr = nullptr;
+        CK(cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal));
+        const int r = body(*b, cap);
+        const cudaError_t e = cudaStreamEndCapture(cap, &gr);
+        if (r != W2L_OK) { if (gr) cudaGraphDestroy(gr); cudaGetLastError(); return r; }
+        CK(e);
+        const cudaError_t ei = cudaGraphInstantiate(&b->exec.h, gr, 0);
+        cudaGraphDestroy(gr);
+        CK(ei);
+        return W2L_OK;
+    }
+
+    // One step of bucket b over rows [0, n) (n <= b->B): row(k) gives the GroupRow of row k.  Rows past n repeat the
+    // last one and are not pasted.  *id gets the step's id; step_done[*id % kStepEvents] is recorded after it.
+    template <class Row>
+    int step(StepBucket* b, int n, Row row, cudaStream_t st, long long* id) {
+        CKR(acquire(b));
+        *id = count++;
+        const int slot = (int)(*id % kStepSlots);
+        CK(cudaEventSynchronize(table_done[slot]));       // its previous copy has read the staging slot
+        waits++;
+        GroupRow* h = (GroupRow*)table_host.p + (size_t)slot * max_batch;
+        for (int k = 0; k < b->B; ++k) {
+            if (k < n) h[k] = row(k);
+            else { h[k] = h[n - 1]; h[k].dst = nullptr; }
+        }
+        CK(cudaMemcpyAsync(table, h, (size_t)b->B * sizeof(GroupRow), cudaMemcpyHostToDevice, st));
+        CK(cudaEventRecord(table_done[slot], st));
+        calls += 2;
+        if (!ctx->use_stream_graph || !b->warm) {
+            CKR(body(*b, st));
+            b->warm = true;
+        } else {
+            if (!b->exec.h) CKR(capture(b));
+            CK(cudaGraphLaunch(b->exec.h, st));
+            calls++;
+        }
+        CK(cudaEventRecord(step_done[*id % kStepEvents], st));   // its gather has read the mel rings
+        calls++;
+        return W2L_OK;
+    }
+};
+
+// a row (W2L_STREAM_ROW ints) of a session with mel ring m, video frames and description d, pasted into dst
+static GroupRow step_row(const MelRing& m, const uint8_t* frames, const w2l_stream_desc& d, const int32_t* r, uint8_t* dst) {
+    GroupRow g;
+    g.mel = m.mel; g.pitch = m.rm; g.start = r[1];
+    g.frames = frames; g.dst = dst;
+    g.H = d.H; g.W = d.W; g.frame = r[2];
+    g.y1 = r[3]; g.y2 = r[4]; g.x1 = r[5]; g.x2 = r[6]; g.pad = 0;
+    return g;
+}
+
+// The steps that read a session's mel ring.  Before the ring kernel writes frames [f_next, f_end) into columns that
+// held frames below f_end - rm, the mel stream waits for the last queued step that reads such a frame.  Steps read
+// from their lowest chunk start upwards and a session's starts never decrease from step to step, so that step is the
+// newest one whose lowest start is below the cutoff.
+struct RingReaders {
+    long long first_lo = -1;                          // the lowest mel frame of the session's first step
+    long long step[kReaderTrack], lo[kReaderTrack];   // its last steps and their lowest mel frames, oldest first
+    int n = 0;
+
+    void track(long long id, long long start) {
+        if (first_lo < 0) first_lo = start;
+        if (n > 0 && step[n - 1] == id) return;   // rows of one step: the first has the lowest start
+        if (n == kReaderTrack) {
+            for (int k = 1; k < kReaderTrack; ++k) { step[k - 1] = step[k]; lo[k - 1] = lo[k]; }
+            --n;
+        }
+        step[n] = id; lo[n] = start; ++n;
+    }
+
+    // The step to wait for before frames below f_end are written into a ring of rm columns (-1: none).  When it is
+    // older than the steps remembered, the oldest remembered one (after it on the caller's stream) stands in for it.
+    long long reader(long long f_end, long long rm) const {
+        const long long cutoff = f_end - rm;
+        if (n == 0 || cutoff <= first_lo) return -1;
+        int k = n - 1;
+        while (k > 0 && lo[k] >= cutoff) --k;
+        return step[k];
+    }
+};
+
+// The video of a session: device memory on the context's device, frames under 2^31 bytes (the paste's offsets within
+// a frame are 32-bit), and the generator to run on it loaded.
+static int check_stream_frames(const w2l_ctx* ctx, const uint8_t* frames, const w2l_stream_desc& d) {
+    if ((long long)d.H * d.W * 3 > INT32_MAX) return fail(W2L_EINVAL, "a %dx%d frame: need fewer than 2^31 bytes", d.H, d.W);
+    cudaPointerAttributes pa;
+    const cudaError_t e = cudaPointerGetAttributes(&pa, frames);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(W2L_EINVAL, "frames: cudaPointerGetAttributes: %s", cudaGetErrorString(e)); }
+    if (pa.type != cudaMemoryTypeDevice || pa.device != ctx->device)
+        return fail(W2L_EINVAL, "frames must be device memory of the context's device %d", ctx->device);
+    if (!ctx->nets[W2L_NET_GENERATOR].loaded) return fail(W2L_ESTATE, "generator weights not loaded");
+    return W2L_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // the session
 // ------------------------------------------------------------------------------------------------
-constexpr int kStreamSlots = 4;   // pinned staging rows of the per-step table in flight
-
 struct w2l_stream {
     w2l_ctx* ctx = nullptr;
     StreamSched sched;
     MelRing mel;
     const uint8_t* frames = nullptr;
-    int batch = 0;
     long long emitted = 0;          // rows whose step has been queued
-    bool nan = false, finished = false;
-    // per-step device table: [batch][5] (frame, y1, y2, x1, x2) for crop and paste, then [batch] chunk starts
-    DevMem<int> table;
-    PinnedMem stage;                // kStreamSlots x the table
-    Event slot_done[kStreamSlots];  // the H2D copy out of each staging slot
+    bool nan = false;
     // The mel work (audio copy, ring kernel, NaN flag read-back) runs on a private stream, so that the host, which waits
     // for each piece's NaN flag before it schedules rows, waits for this session's mel frames only, not for the steps
-    // queued on the caller's stream.  The ring kernel overwrites mel columns that queued steps may still read: before
-    // it runs, the mel stream waits for the last step that reads a column it overwrites (step_done / step_lo).
+    // queued on the caller's stream.
     Stream s_mel;
     Event ev_caller;                // the caller's stream, before a piece of device audio is copied
-    Event step_done[kStreamSlots];  // recorded after the gather of step k (slot k % kStreamSlots) on the caller's stream
-    long long step_lo[kStreamSlots] = {0, 0, 0, 0};   // the lowest mel frame step k reads
-    long long first_lo = -1;        // that of the session's first step
-    long long steps = 0;
-    DevMem<float> chunks;
-    DevMem<uint8_t> crops, preds;
-    // the generator plan the step replays, pinned against LRU eviction while held; valid while epoch matches
-    Plan* plan = nullptr;
-    uint64_t epoch = 0;
-    Stream cap;                     // capture stream (the graph is launched on the caller's stream)
-    GraphExec exec;
-    bool warm = false;              // one uncaptured step ran on the current plan (kernel attributes are set)
+    StepRunner steps;
+    StepBucket bucket;              // every step runs at B = batch
+    RingReaders readers;
 };
 
-static void stream_release_plan(w2l_stream* s) {
-    if (s->plan && s->epoch == s->ctx->plan_epoch[W2L_NET_GENERATOR]) s->plan->pins--;
-    s->plan = nullptr;
-    s->exec.reset();
-    s->warm = false;
-}
-
-// The plan is erased, with every generator plan, only by drop_plans (new weights), which bumps the epoch; LRU eviction
-// skips pinned plans.  So a matching epoch means the plan, and every buffer the graph bakes, is alive and current.
-static int stream_acquire_plan(w2l_stream* s) {
-    w2l_ctx* ctx = s->ctx;
-    if (s->plan && s->epoch == ctx->plan_epoch[W2L_NET_GENERATOR]) return W2L_OK;
-    stream_release_plan(s);
-    Plan* pl;
-    CKR(get_plan(ctx, W2L_NET_GENERATOR, s->batch, 0, &pl));
-    pl->pins++;
-    s->plan = pl;
-    s->epoch = ctx->plan_epoch[W2L_NET_GENERATOR];
-    return W2L_OK;
-}
-
-// gather + crop/resize + generator: every argument is a session buffer, so the launches can be captured once
-static int stream_body(w2l_stream* s, cudaStream_t st) {
-    w2l_ctx* ctx = s->ctx;
-    const int B = s->batch;
-    const StreamSched& sc = s->sched;
-    mel_ring_gather_kernel<<<(B * 1280 + 255) / 256, 256, 0, st>>>(s->mel.mel, s->mel.rm, s->table.p + 5 * B, B, s->chunks);
-    const long long total = (long long)B * 96 * 96;
-    crop_resize_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16), 256, 0, st>>>(
-        s->frames, sc.d.H, sc.d.W, s->table, B, 96, s->crops);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    return run_plan(ctx, s->plan, s->chunks, s->crops, s->preds, nullptr, st, true);
-}
-
-static int stream_capture(w2l_stream* s) {
-    cudaGraph_t g = nullptr;
-    CK(cudaStreamBeginCapture(s->cap, cudaStreamCaptureModeThreadLocal));
-    const int r = stream_body(s, s->cap);
-    const cudaError_t e = cudaStreamEndCapture(s->cap, &g);
-    if (r != W2L_OK) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return r; }
-    CK(e);
-    const cudaError_t ei = cudaGraphInstantiate(&s->exec.h, g, 0);
-    cudaGraphDestroy(g);
-    CK(ei);
-    return W2L_OK;
-}
-
-// one generator step over rows[0, n) (n <= batch), output frames to out (n, H, W, 3)
-static int stream_step(w2l_stream* s, const int32_t* rows, int n, uint8_t* out, cudaStream_t st) {
-    w2l_ctx* ctx = s->ctx;
-    const int B = s->batch;
-    CKR(stream_acquire_plan(s));
-    const int slot = (int)(s->steps++ % kStreamSlots);
-    CK(cudaEventSynchronize(s->slot_done[slot]));       // its previous copy has read the staging row
-    int32_t* h = (int32_t*)s->stage.p + (size_t)slot * B * 6;
-    for (int b = 0; b < B; ++b) {
-        const int32_t* r = rows + W2L_STREAM_ROW * std::min(b, n - 1);   // rows past n repeat the last one
-        h[5 * b + 0] = r[2]; h[5 * b + 1] = r[3]; h[5 * b + 2] = r[4]; h[5 * b + 3] = r[5]; h[5 * b + 4] = r[6];
-        h[5 * B + b] = r[1];
+// Full batches of pend run (all: and the rest, in one step padded to the batch); output frames go to out from row first.
+static int stream_flush(w2l_stream* s, std::vector<int32_t>* pend, uint8_t* out, long long first, bool all, cudaStream_t st) {
+    const size_t frame_bytes = (size_t)s->sched.d.H * s->sched.d.W * 3;
+    const size_t B = (size_t)s->bucket.B;
+    while (pend->size() >= B * W2L_STREAM_ROW || (all && !pend->empty())) {
+        const int n = (int)std::min(B, pend->size() / W2L_STREAM_ROW);
+        const int32_t* rows = pend->data();
+        uint8_t* o = out + (size_t)(s->emitted - first) * frame_bytes;
+        long long id;
+        CKR(s->steps.step(&s->bucket, n, [&](int k) {
+            return step_row(s->mel, s->frames, s->sched.d, rows + (size_t)k * W2L_STREAM_ROW, o + (size_t)k * frame_bytes);
+        }, st, &id));
+        s->readers.track(id, rows[1]);   // rows are in output order: the first has the lowest start
+        s->emitted += n;
+        pend->erase(pend->begin(), pend->begin() + (size_t)n * W2L_STREAM_ROW);
     }
-    CK(cudaMemcpyAsync(s->table, h, (size_t)B * 6 * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaEventRecord(s->slot_done[slot], st));
-    if (!ctx->use_stream_graph || !s->warm) {
-        CKR(stream_body(s, st));
-        s->warm = true;
-    } else {
-        if (!s->exec.h) CKR(stream_capture(s));
-        CK(cudaGraphLaunch(s->exec.h, st));
-    }
-    CK(cudaEventRecord(s->step_done[slot], st));      // its gather has read the mel ring
-    s->step_lo[slot] = rows[1];                        // rows are in output order: the first has the lowest start
-    if (s->first_lo < 0) s->first_lo = rows[1];
-    // the paste writes into the caller's buffer and only the n real rows: launched outside the graph
-    const StreamSched& sc = s->sched;
-    const long long total = (long long)n * sc.d.H * sc.d.W;
-    paste_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 32), 256, 0, st>>>(
-        s->preds, 96, s->frames, sc.d.H, sc.d.W, s->table, n, out);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    s->emitted += n;
-    return W2L_OK;
-}
-
-// Before the ring kernel writes frames [f_next, f_end) into columns that held frames below f_end - rm: make the mel
-// stream wait for the last queued step that reads such a frame.  Steps read from their lowest chunk start upwards and
-// those starts never decrease from step to step, so that step is the newest one with step_lo < cutoff; if it is older
-// than the tracked slots, the oldest tracked step (after it on the caller's stream) stands in for it.
-static int stream_wait_readers(w2l_stream* s, long long f_end) {
-    const long long cutoff = f_end - s->mel.rm;
-    if (s->steps == 0 || cutoff <= s->first_lo) return W2L_OK;
-    const long long tracked = std::min<long long>(s->steps, kStreamSlots);
-    long long k = s->steps - 1;
-    while (k > s->steps - tracked && s->step_lo[k % kStreamSlots] >= cutoff) --k;
-    CK(cudaStreamWaitEvent(s->s_mel, s->step_done[k % kStreamSlots], 0));
-    return W2L_OK;
-}
-
-// mel frames up to f_end on the mel stream, then the NaN flag; the caller's stream is ordered after them
-static int stream_mel(w2l_stream* s, const MelParams& tables, long long f_end, long long L_end, cudaStream_t st) {
-    CKR(stream_wait_readers(s, f_end));
-    CKR(s->mel.compute(tables, f_end, L_end, s->s_mel));
-    bool nan;
-    CKR(s->mel.nan_seen(s->s_mel, &nan));     // before any row reads the new frames (and the audio copy is done)
-    if (nan) { s->nan = true; return fail(W2L_EINVAL, "%s", kMelNanMsg); }
-    CK(cudaStreamWaitEvent(st, s->mel.ev_nan, 0));
     return W2L_OK;
 }
 
@@ -525,27 +637,10 @@ static int stream_pending(const w2l_stream* s, long long n_samples, bool finish,
     return W2L_OK;
 }
 
-// rows [s->emitted + pend, a.n_fixed) join pend; full batches of pend run
-static int stream_advance(w2l_stream* s, const StreamSched::At& a, std::vector<int32_t>* pend, uint8_t* out,
-                          long long first, cudaStream_t st) {
-    const size_t frame_bytes = (size_t)s->sched.d.H * s->sched.d.W * 3;
-    long long next = s->emitted + (long long)(pend->size() / W2L_STREAM_ROW);
-    for (; next < a.n_fixed; ++next) {
-        int32_t r[W2L_STREAM_ROW];
-        CKR(s->sched.row(next, a, r));
-        pend->insert(pend->end(), r, r + W2L_STREAM_ROW);
-    }
-    while ((long long)(pend->size() / W2L_STREAM_ROW) >= s->batch) {
-        CKR(stream_step(s, pend->data(), s->batch, out + (size_t)(s->emitted - first) * frame_bytes, st));
-        pend->erase(pend->begin(), pend->begin() + (size_t)s->batch * W2L_STREAM_ROW);
-    }
-    return W2L_OK;
-}
-
 static int stream_run(w2l_stream* s, const float* pcm, long long n, bool finish, uint8_t* out, long long cap,
                       long long* first_index, long long* n_out, cudaStream_t st) {
     if (s->nan) return fail(W2L_EINVAL, "%s", kMelNanMsg);
-    if (s->finished) return fail(W2L_ESTATE, "the stream is finished");
+    if (s->mel.finished) return fail(W2L_ESTATE, "the stream is finished");
     if (n < 0 || (n > 0 && !pcm)) return fail(W2L_EINVAL, "bad audio piece (%lld samples)", n);
     long long need;
     CKR(stream_pending(s, n, finish, &need));
@@ -563,33 +658,31 @@ static int stream_run(w2l_stream* s, const float* pcm, long long n, bool finish,
             CK(cudaStreamWaitEvent(s->s_mel, s->ev_caller, 0));
         }
     }
+    MelRing& m = s->mel;
     std::vector<int32_t> pend;
-    StreamSched::At a;
-    long long done = 0;
-    while (done < n) {
-        const long long keep = std::min(s->mel.f_next, s->sched.start(s->emitted));
-        const long long room = s->mel.max_piece(keep);
-        const long long piece = std::min(n - done, s->mel.max_input(room));
-        if (piece <= 0) return fail(W2L_ESTATE, "mel ring too small for the pending rows");
-        CKR(s->mel.feed(pcm + done, piece, room, s->s_mel));
-        done += piece;
-        CKR(stream_mel(s, tables, mel_final_frames(s->mel.L), -1, st));
-        CKR(s->sched.at(s->mel.L, false, &a));
-        CKR(stream_advance(s, a, &pend, out, first, st));
+    std::vector<double> starts;
+    for (long long done = 0; done < n || (finish && !m.finished); ) {
+        MelPiece p;
+        CKR(m.plan(n - done, finish, std::min(m.f_next, s->sched.start(s->emitted)), &p, &starts));
+        const long long rd = s->readers.reader(p.f_end, m.rm);
+        CKR(m.launch(p, pcm + done, starts, tables, rd >= 0 ? (cudaEvent_t)s->steps.step_done[rd % kStepEvents] : nullptr,
+                     s->s_mel));
+        m.commit(p);
+        done += p.n;
+        bool nan;
+        CKR(m.nan_seen(s->s_mel, &nan));     // before any row reads the new frames (and the audio copy is done)
+        if (nan) { s->nan = true; return fail(W2L_EINVAL, "%s", kMelNanMsg); }
+        CK(cudaStreamWaitEvent(st, m.ev_nan, 0));
+        StreamSched::At a;
+        CKR(s->sched.at(m.L, p.fin, &a));
+        for (long long i = s->emitted + (long long)(pend.size() / W2L_STREAM_ROW); i < a.n_fixed; ++i) {
+            int32_t r[W2L_STREAM_ROW];
+            CKR(s->sched.row(i, a, r));
+            pend.insert(pend.end(), r, r + W2L_STREAM_ROW);
+        }
+        CKR(stream_flush(s, &pend, out, first, false, st));
     }
-    if (finish) {
-        CKR(s->mel.end_input(s->mel.max_piece(std::min(s->mel.f_next, s->sched.start(s->emitted))), s->s_mel));
-        CKR(s->sched.at(s->mel.L, true, &a));
-        const long long keep = std::min(std::min(s->mel.f_next, s->sched.start(s->emitted)), a.M - 16);
-        if (a.M - keep > s->mel.rm) return fail(W2L_ESTATE, "mel ring too small for the pending rows");
-        CKR(stream_mel(s, tables, a.M, s->mel.L, st));
-        CKR(stream_advance(s, a, &pend, out, first, st));
-        s->finished = true;
-    }
-    if (!pend.empty()) {
-        const size_t frame_bytes = (size_t)s->sched.d.H * s->sched.d.W * 3;
-        CKR(stream_step(s, pend.data(), (int)(pend.size() / W2L_STREAM_ROW), out + (size_t)(s->emitted - first) * frame_bytes, st));
-    }
+    CKR(stream_flush(s, &pend, out, first, true, st));
     *n_out = s->emitted - first;
     return W2L_OK;
 }
@@ -632,23 +725,14 @@ static int melstream_run(w2l_melstream* ms, const float* pcm, long long n, bool 
     int kind = PCM_PAGEABLE;
     if (n > 0) CKR(pcm_kind(ms->ctx, pcm, &kind));
     const long long first = r.f_next;
-    long long done = 0;
-    while (done < n) {
-        const long long room = r.max_piece(r.f_next);
-        const long long piece = std::min(n - done, r.max_input(room));
-        if (piece <= 0) return fail(W2L_ESTATE, "audio ring too small for the resampling");
-        CKR(r.feed(pcm + done, piece, room, st));
-        done += piece;
-        const long long a = r.f_next;
-        CKR(r.compute(tables, mel_final_frames(r.L), -1, st));
-        CKR(r.copy_out(a, r.f_next, mel_out, need, a - first, st));
-    }
-    if (finish) {
-        CKR(r.end_input(r.max_piece(r.f_next), st));
-        const long long a = r.f_next;
-        CKR(r.compute(tables, 1 + r.L / MEL_HOP, r.L, st));
-        CKR(r.copy_out(a, r.f_next, mel_out, need, a - first, st));
-        r.finished = true;
+    std::vector<double> starts;
+    for (long long done = 0; done < n || (finish && !r.finished); ) {
+        MelPiece p;
+        CKR(r.plan(n - done, finish, r.f_next, &p, &starts));
+        CKR(r.launch(p, pcm + done, starts, tables, nullptr, st));
+        CKR(r.copy_out(r.f_next, p.f_end, mel_out, need, r.f_next - first, st));
+        r.commit(p);
+        done += p.n;
     }
     *n_new = r.f_next - first;
     if (kind == PCM_PINNED) {   // the copies read pinned memory when they run: let the caller reuse it on return
@@ -718,26 +802,14 @@ int w2l_stream_create(w2l_ctx* ctx, const uint8_t* frames_dev, const w2l_stream_
     s->ctx = ctx;
     CKR(s->sched.init(d, rects_host));
     DeviceGuard g(ctx->device);
-    cudaPointerAttributes pa;
-    const cudaError_t e = cudaPointerGetAttributes(&pa, frames_dev);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(W2L_EINVAL, "frames: cudaPointerGetAttributes: %s", cudaGetErrorString(e)); }
-    if (pa.type != cudaMemoryTypeDevice || pa.device != ctx->device)
-        return fail(W2L_EINVAL, "frames must be device memory of the context's device %d", ctx->device);
-    if (!ctx->nets[W2L_NET_GENERATOR].loaded) return fail(W2L_ESTATE, "generator weights not loaded");
+    CKR(check_stream_frames(ctx, frames_dev, *d));
     s->frames = frames_dev;
-    s->batch = batch;
+    s->bucket.B = batch;
     // the mel ring holds the frames of every row not yet run (< batch + 4 chunks) beside a whole audio ring of new ones
     CKR(s->mel.init(ctx, 0, (long long)std::ceil((batch + 4) * s->sched.mult) + 64 + (1LL << 16) / MEL_HOP + 16));
-    CKR(s->table.grow(ctx, (size_t)batch * 6 * 4));
-    CKR(s->stage.alloc((size_t)kStreamSlots * batch * 6 * 4));
-    for (Event& ev : s->slot_done) CKR(ev.create());
-    for (Event& ev : s->step_done) CKR(ev.create());
+    CKR(s->steps.init(ctx, batch));
     CKR(s->ev_caller.create());
     CKR(s->s_mel.create());
-    CKR(s->chunks.grow(ctx, (size_t)batch * 1280 * 4));
-    CKR(s->crops.grow(ctx, (size_t)batch * 96 * 96 * 3));
-    CKR(s->preds.grow(ctx, (size_t)batch * 96 * 96 * 3));
-    CKR(s->cap.create());
     *out = s.release();
     return W2L_OK;
 }
@@ -745,7 +817,7 @@ int w2l_stream_create(w2l_ctx* ctx, const uint8_t* frames_dev, const w2l_stream_
 int w2l_stream_pending(const w2l_stream* s, int64_t n_samples, int finish, int64_t* n_out) {
     if (!s || !n_out || n_samples < 0) return fail(W2L_EINVAL, "bad argument");
     if (s->nan) return fail(W2L_EINVAL, "%s", kMelNanMsg);
-    if (s->finished) { *n_out = 0; return W2L_OK; }
+    if (s->mel.finished) { *n_out = 0; return W2L_OK; }
     long long n;
     CKR(stream_pending(s, n_samples, finish != 0, &n));
     *n_out = n;
@@ -779,7 +851,7 @@ int w2l_stream_destroy(w2l_stream* s) {
     if (!s) return W2L_OK;
     DeviceGuard g(s->ctx->device);
     cudaDeviceSynchronize();   // queued steps may still read the session's buffers
-    stream_release_plan(s);
+    s->steps.release(&s->bucket);
     delete s;
     return W2L_OK;
 }

@@ -6,10 +6,6 @@
 // Part of the single translation unit w2l_api.cu (included there, after host_stream.cuh).
 #pragma once
 
-constexpr int kGroupSlots = 4;         // pinned staging slots of the per-step table in flight
-constexpr int kGroupStepEvents = 16;   // step-completion events the ring-safety wait chooses from
-constexpr int kGroupTrack = 4;         // the last steps each session remembers (step id, lowest chunk start)
-
 // Bucket sizes: powers of two below max_batch, then max_batch.  n rows run as full max_batch steps, then the remainder
 // in the smallest bucket that holds it.  Host only (w2l_stream_group_buckets).
 static int group_bucket(int max_batch, long long n) {
@@ -36,44 +32,13 @@ struct GroupSession {
     MelRing mel;
     const uint8_t* frames = nullptr;
     long long emitted = 0;           // rows whose step has been queued
-    bool failed = false, finished = false;
+    bool failed = false;
     std::string msg;                 // why it failed: the NaN message, or a detection's
     bool detect = false;             // rects found by the group's detector
     long long det_launched = 0;      // frames [0, det_launched) have a detection queued or read back
     long long det_ok = 0;            // frames [0, det_ok) were read back with a face
     std::vector<int8_t> det_status;  // per frame: -1 not read back yet, else kRectFace / kRectNone / kRectNonFinite
-    long long first_lo = -1;         // the lowest mel frame of its first step
-    long long trk_step[kGroupTrack], trk_lo[kGroupTrack];   // its last steps, oldest first
-    int n_trk = 0;
-
-    void track(long long step, long long lo) {
-        if (first_lo < 0) first_lo = lo;
-        if (n_trk > 0 && trk_step[n_trk - 1] == step) return;   // rows of one step: the first has the lowest start
-        if (n_trk == kGroupTrack) {
-            for (int k = 1; k < kGroupTrack; ++k) { trk_step[k - 1] = trk_step[k]; trk_lo[k - 1] = trk_lo[k]; }
-            --n_trk;
-        }
-        trk_step[n_trk] = step; trk_lo[n_trk] = lo; ++n_trk;
-    }
-
-    // The step the mel stream must wait for before the ring kernel writes frames below f_end (-1: none), as
-    // stream_wait_readers: the newest step that reads a frame below f_end - rm; when it is older than the steps
-    // remembered, the oldest remembered one (after it on the caller's stream) stands in for it.
-    long long reader(long long f_end) const {
-        const long long cutoff = f_end - mel.rm;
-        if (n_trk == 0 || cutoff <= first_lo) return -1;
-        int k = n_trk - 1;
-        while (k > 0 && trk_lo[k] >= cutoff) --k;
-        return trk_step[k];
-    }
-};
-
-struct GroupBucket {
-    int B = 0;
-    Plan* plan = nullptr;            // pinned while held; valid while epoch matches
-    uint64_t epoch = 0;
-    GraphExec exec;
-    bool warm = false;               // one uncaptured step ran on the current plan (kernel attributes are set)
+    RingReaders readers;             // the steps that read its mel ring, among the group's
 };
 
 // an S3FD plan of one (H, W, B), pinned while a detecting session of that frame size is open; valid while epoch matches
@@ -97,7 +62,7 @@ struct DetJob {
 
 struct w2l_stream_group {
     w2l_ctx* ctx = nullptr;
-    int max_batch = 0, ring_log2 = 0;
+    int ring_log2 = 0;
     std::map<int32_t, std::unique_ptr<GroupSession>> sessions;
     int32_t next_id = 0;
     std::vector<int> free_slots;
@@ -115,18 +80,8 @@ struct w2l_stream_group {
     // the steps queued on the caller's stream.
     Stream s_mel;
     Event ev_mel, ev_caller;
-    // the step table: one device table (max_batch rows) shared by every bucket, filled from a pinned slot per step
-    DevMem<GroupRow> table;
-    PinnedMem table_host;            // kGroupSlots x max_batch rows
-    Event table_done[kGroupSlots];
-    Event step_done[kGroupStepEvents];   // after step k (k % kGroupStepEvents) on the caller's stream
-    long long steps = 0;
-    DevMem<float> chunks;
-    DevMem<uint8_t> crops, preds;
-    std::vector<std::unique_ptr<GroupBucket>> buckets;
-    Stream cap;                      // capture stream
-    int64_t calls = 0, waits = 0;    // CUDA API submissions (launches, graph launches, copies, event records and waits)
-                                     // and host synchronisations made by ticks
+    StepRunner steps;                // at max_batch; its counters count every call and host wait of the ticks
+    std::vector<std::unique_ptr<StepBucket>> buckets;
     // Face detection runs on a stream of its own; ev_det follows the last launch.  Every launch is read back by the
     // next round's host wait (the mel stream waits for ev_det before its NaN read-back), so jobs are busy until then.
     Stream s_det;
@@ -200,7 +155,7 @@ static int group_det_launch(w2l_stream_group* g, const std::pair<GroupSession*, 
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync((uint8_t*)j->host.p + kDetHostRects, dv + kDetDevRects, (size_t)n * 5 * 4, cudaMemcpyDeviceToHost, g->s_det));
-    g->calls += 2 + (ctx->launches - l0);
+    g->steps.calls += 2 + (ctx->launches - l0);
     g->det_busy.push_back(std::move(j));
     return W2L_OK;
 }
@@ -225,7 +180,7 @@ static int group_detect(w2l_stream_group* g, const std::vector<std::pair<GroupSe
     }
     for (const auto& u : upto) u.first->det_launched = std::max(u.first->det_launched, u.second);
     CK(cudaEventRecord(g->ev_det, g->s_det));
-    g->calls++;
+    g->steps.calls++;
     return W2L_OK;
 }
 
@@ -262,62 +217,11 @@ static bool group_det_failed(GroupSession* s, long long n, std::string* msg) {
     return true;
 }
 
-static void group_release(w2l_stream_group* g, GroupBucket* b) {
-    if (b->plan && b->epoch == g->ctx->plan_epoch[W2L_NET_GENERATOR]) b->plan->pins--;
-    b->plan = nullptr;
-    b->exec.reset();
-    b->warm = false;
-}
-
-static GroupBucket* group_bucket_of(w2l_stream_group* g, int B) {
+static StepBucket* group_bucket_of(w2l_stream_group* g, int B) {
     for (auto& b : g->buckets) if (b->B == B) return b.get();
-    g->buckets.emplace_back(new GroupBucket());
+    g->buckets.emplace_back(new StepBucket());
     g->buckets.back()->B = B;
     return g->buckets.back().get();
-}
-
-// as stream_acquire_plan, per bucket
-static int group_acquire(w2l_stream_group* g, GroupBucket* b) {
-    w2l_ctx* ctx = g->ctx;
-    if (b->plan && b->epoch == ctx->plan_epoch[W2L_NET_GENERATOR]) return W2L_OK;
-    group_release(g, b);
-    Plan* pl;
-    CKR(get_plan(ctx, W2L_NET_GENERATOR, b->B, 0, &pl));
-    pl->pins++;
-    b->plan = pl;
-    b->epoch = ctx->plan_epoch[W2L_NET_GENERATOR];
-    return W2L_OK;
-}
-
-// gather + crop + generator + paste of B table rows: every argument is a group buffer, so the launches are captured
-static int group_body(w2l_stream_group* g, GroupBucket* b, cudaStream_t st) {
-    w2l_ctx* ctx = g->ctx;
-    const int B = b->B;
-    group_gather_kernel<<<(B * 1280 + 255) / 256, 256, 0, st>>>(g->table, B, g->chunks);
-    const long long total = (long long)B * 96 * 96;
-    group_crop_kernel<<<(int)std::min<long long>((total + 255) / 256, ctx->num_sms * 16), 256, 0, st>>>(g->table, B, 96, g->crops);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    CKR(run_plan(ctx, b->plan, g->chunks, g->crops, g->preds, nullptr, st, true));
-    // about 8 blocks per SM over the step, each row's frame split across gridDim.x of them
-    const dim3 grid((unsigned)std::max(1, (ctx->num_sms * 8 + B - 1) / B), (unsigned)B);
-    group_paste_kernel<<<grid, 256, 0, st>>>(g->preds, 96, g->table);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    return W2L_OK;
-}
-
-static int group_capture(w2l_stream_group* g, GroupBucket* b) {
-    cudaGraph_t gr = nullptr;
-    CK(cudaStreamBeginCapture(g->cap, cudaStreamCaptureModeThreadLocal));
-    const int r = group_body(g, b, g->cap);
-    const cudaError_t e = cudaStreamEndCapture(g->cap, &gr);
-    if (r != W2L_OK) { if (gr) cudaGraphDestroy(gr); cudaGetLastError(); return r; }
-    CK(e);
-    const cudaError_t ei = cudaGraphInstantiate(&b->exec.h, gr, 0);
-    cudaGraphDestroy(gr);
-    CK(ei);
-    return W2L_OK;
 }
 
 // one pooled row of a tick: the session, its row (W2L_STREAM_ROW ints) and its output frame
@@ -329,39 +233,13 @@ struct GroupPend {
 
 // one step over pend[0, n) (n <= max_batch) in the smallest bucket that holds it
 static int group_step(w2l_stream_group* g, const GroupPend* pend, int n, cudaStream_t st) {
-    w2l_ctx* ctx = g->ctx;
-    GroupBucket* b = group_bucket_of(g, group_bucket(g->max_batch, n));
-    CKR(group_acquire(g, b));
-    const long long id = g->steps++;
-    const int slot = (int)(id % kGroupSlots);
-    CK(cudaEventSynchronize(g->table_done[slot]));       // its previous copy has read the staging slot
-    g->waits++;
-    GroupRow* h = (GroupRow*)g->table_host.p + (size_t)slot * g->max_batch;
-    for (int k = 0; k < b->B; ++k) {
-        const GroupPend& p = pend[std::min(k, n - 1)];    // rows past n repeat the last one and are not pasted
-        const GroupSession* s = p.s;
-        const int32_t* r = p.row;
-        GroupRow& d = h[k];
-        d.mel = s->mel.mel; d.pitch = s->mel.rm; d.start = r[1];
-        d.frames = s->frames; d.dst = k < n ? p.dst : nullptr;
-        d.H = s->sched.d.H; d.W = s->sched.d.W; d.frame = r[2];
-        d.y1 = r[3]; d.y2 = r[4]; d.x1 = r[5]; d.x2 = r[6]; d.pad = 0;
-    }
-    CK(cudaMemcpyAsync(g->table, h, (size_t)b->B * sizeof(GroupRow), cudaMemcpyHostToDevice, st));
-    CK(cudaEventRecord(g->table_done[slot], st));
-    g->calls += 2;
-    if (!ctx->use_stream_graph || !b->warm) {
-        CKR(group_body(g, b, st));
-        b->warm = true;
-    } else {
-        if (!b->exec.h) CKR(group_capture(g, b));
-        CK(cudaGraphLaunch(b->exec.h, st));
-        g->calls++;
-    }
-    CK(cudaEventRecord(g->step_done[id % kGroupStepEvents], st));   // its gather has read the mel rings
-    g->calls++;
+    long long id;
+    CKR(g->steps.step(group_bucket_of(g, group_bucket(g->steps.max_batch, n)), n, [&](int k) {
+        const GroupPend& p = pend[k];
+        return step_row(p.s->mel, p.s->frames, p.s->sched.d, p.row, p.dst);
+    }, st, &id));
     for (int k = 0; k < n; ++k) {
-        pend[k].s->track(id, pend[k].row[1]);
+        pend[k].s->readers.track(id, pend[k].row[1]);
         pend[k].s->emitted++;
     }
     return W2L_OK;
@@ -413,9 +291,8 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
                        cudaStream_t st, bool* more) {
     w2l_ctx* ctx = g->ctx;
     const MelParams tables = mel_tables(ctx);
-    // piece: input samples; L: the 16 kHz count after it (resampling sessions: the outputs it makes final, clk their clock)
-    struct Plan1 { long long piece, f_end, L_end, L; bool fin; ResampleClock clk; };
-    std::vector<Plan1> pl(items.size());
+    std::vector<MelPiece> pl(items.size());
+    std::vector<char> live(items.size(), 0);   // the item has a piece this round
     std::vector<GroupScatter> sc;
     std::vector<MelGroupBlock> mb;
     std::vector<ResampleGroupBlock> rb;
@@ -425,66 +302,30 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
     long long wait_step = -1;
     for (size_t i = 0; i < items.size(); ++i) {
         GroupItem& it = items[i];
-        Plan1& p = pl[i];
-        p = Plan1{0, 0, -1, -1, false, ResampleClock()};   // L < 0: no work this round
-        if (!it.s || it.failed || it.s->finished) continue;
+        if (!it.s || it.failed || it.s->mel.finished) continue;
         GroupSession* s = it.s;
         if (it.done == it.n && !it.finish) continue;
         MelRing& m = s->mel;
-        const long long keep = std::min(m.f_next, s->sched.start(s->emitted));
-        const long long room = m.max_piece(keep);
-        p.piece = std::min(it.n - it.done, m.max_input(room));
-        if (it.n > it.done && p.piece <= 0) return fail(W2L_ESTATE, "session %d: mel ring too small for the pending rows", s->id);
-        bool end_in = it.finish && it.done + p.piece == it.n;   // the input ends with this piece
-        p.L = m.L + p.piece;
-        if (m.resampling()) {
-            // the outputs the piece makes final; the input's end adds the rest once they fit the rings (else a later round)
-            starts.clear();
-            p.clk = m.clk;
-            p.L = p.clk.advance(m.n_in + p.piece, end_in, &starts);
-            if (end_in && p.L - m.L > room) {
-                starts.clear();
-                p.clk = m.clk;
-                p.L = p.clk.advance(m.n_in + p.piece, false, &starts);
-                end_in = false;
-            }
-            const long long n_in = m.n_in + p.piece;
-            for (size_t b = 0; b < starts.size(); ++b) {
-                ResampleGroupBlock blk;
-                blk.p = resample_params(m.clk, m.wd, nullptr, m.L, p.L, end_in ? m.clk.n_res(n_in) : (1LL << 62));
-                blk.r.src = m.src; blk.r.src_mask = m.rsrc - 1; blk.r.n_in = end_in ? n_in : (1LL << 62);
-                blk.r.audio = m.audio; blk.r.audio_mask = m.ra - 1; blk.r.nan = g->nan.p + s->slot;
-                blk.tb = m.L + (long long)b * RS_THREADS;
-                blk.reg = starts[b];
-                rb.push_back(blk);
-            }
+        MelPiece& p = pl[i];
+        if (m.plan(it.n - it.done, it.finish, std::min(m.f_next, s->sched.start(s->emitted)), &p, &starts) != W2L_OK)
+            return fail(W2L_ESTATE, "session %d: %s", s->id, g_err.c_str());
+        live[i] = any = true;
+        int* flag = g->nan.p + s->slot;
+        for (size_t b = 0; b < starts.size(); ++b) {   // only when the session resamples
+            ResampleGroupBlock blk;
+            m.resample_args(p, nullptr, flag, &blk.p, &blk.r);
+            blk.tb = m.L + (long long)b * RS_THREADS;
+            blk.reg = starts[b];
+            rb.push_back(blk);
         }
-        const long long L = p.L;
-        p.f_end = mel_final_frames(L);
-        if (end_in) {
-            const long long M = it.last.M;
-            if (M - std::min(keep, M - 16) <= s->mel.rm) { p.fin = true; p.f_end = M; p.L_end = L; }
+        if (p.n > 0) {   // host pcm: an offset into the packed upload until it is packed
+            sc.push_back(m.input_of(p, it.device ? it.pcm + it.done : (const float*)(uintptr_t)host_samples));
+            if (it.device) any_device = true; else host_samples += (size_t)p.n;
         }
-        if (p.piece == 0 && p.L == m.L && !p.fin)
-            return fail(W2L_ESTATE, "session %d: mel ring too small for the pending rows", s->id);
-        any = true;
-        if (p.piece > 0) {   // into the audio ring, or the input ring of a resampling session
-            GroupScatter d;
-            d.src = it.device ? it.pcm + it.done : (const float*)(uintptr_t)host_samples;   // an offset until packed
-            if (m.resampling()) { d.ring = m.src; d.mask = m.rsrc - 1; d.at = m.n_in; }
-            else { d.ring = m.audio; d.mask = m.ra - 1; d.at = m.L; }
-            d.n = p.piece;
-            if (it.device) any_device = true; else host_samples += (size_t)p.piece;
-            sc.push_back(d);
-        }
-        for (long long f = s->mel.f_next; f < p.f_end; f += MEL_FPB) {
-            MelGroupBlock blk;
-            blk.audio = s->mel.audio; blk.audio_mask = s->mel.ra - 1; blk.mel = s->mel.mel; blk.mel_pitch = s->mel.rm;
-            blk.L = p.L_end >= 0 ? p.L_end : (1LL << 62);
-            blk.fb = f; blk.f1 = p.f_end; blk.nan = g->nan.p + s->slot;
-            mb.push_back(blk);
-        }
-        if (p.f_end > s->mel.f_next) wait_step = std::max(wait_step, s->reader(p.f_end));
+        const MelRingParams r = m.mel_args(p, flag);
+        for (long long f = r.f0; f < r.f1; f += MEL_FPB)
+            mb.push_back(MelGroupBlock{r.audio, r.audio_mask, r.mel, r.mel_pitch, r.L, f, r.f1, r.nan});
+        if (p.f_end > m.f_next) wait_step = std::max(wait_step, s->readers.reader(p.f_end, m.rm));
     }
     *more = false;
     if (!any) return W2L_OK;
@@ -500,11 +341,11 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
         size_t k = 0;
         for (size_t i = 0; i < items.size(); ++i) {
             GroupItem& it = items[i];
-            if (pl[i].piece == 0) continue;
+            if (pl[i].n == 0) continue;
             GroupScatter& d = sc[k++];
             if (!it.device) {
                 const size_t at = (size_t)(uintptr_t)d.src;
-                memcpy(hp + o_pcm + at * 4, it.pcm + it.done, (size_t)pl[i].piece * 4);
+                memcpy(hp + o_pcm + at * 4, it.pcm + it.done, (size_t)pl[i].n * 4);
                 d.src = (const float*)(g->up.p + o_pcm) + at;
             }
         }
@@ -513,58 +354,56 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
     memcpy(hp + o_mb, mb.data(), mb.size() * sizeof(MelGroupBlock));
     memcpy(hp + o_rb, rb.data(), rb.size() * sizeof(ResampleGroupBlock));
     CK(cudaMemcpyAsync(g->up, hp, bytes, cudaMemcpyHostToDevice, g->s_mel));
-    g->calls++;
+    g->steps.calls++;
     if (any_device) {   // device audio may be produced by work queued on the caller's stream
         CK(cudaEventRecord(g->ev_caller, st));
         CK(cudaStreamWaitEvent(g->s_mel, g->ev_caller, 0));
-        g->calls += 2;
+        g->steps.calls += 2;
     }
     // the newest queued step that reads a mel column this round overwrites (the steps before it are done by then)
     if (wait_step >= 0) {
-        CK(cudaStreamWaitEvent(g->s_mel, g->step_done[wait_step % kGroupStepEvents], 0));
-        g->calls++;
+        CK(cudaStreamWaitEvent(g->s_mel, g->steps.step_done[wait_step % kStepEvents], 0));
+        g->steps.calls++;
     }
     if (!sc.empty()) {
         long long longest = 0;
         for (const GroupScatter& d : sc) longest = std::max(longest, d.n);
         const dim3 grid((unsigned)std::min<long long>((longest + 255) / 256, 64), (unsigned)sc.size());
         group_scatter_kernel<<<grid, 256, 0, g->s_mel>>>((const GroupScatter*)g->up.p);
-        ctx->launches++; g->calls++;
+        ctx->launches++; g->steps.calls++;
         CK(cudaGetLastError());
     }
     if (!rb.empty()) {   // only when some session resamples: its new outputs into its audio ring
         resample_group_kernel<<<(unsigned)rb.size(), RS_THREADS, 0, g->s_mel>>>((const ResampleGroupBlock*)(g->up.p + o_rb));
-        ctx->launches++; g->calls++;
+        ctx->launches++; g->steps.calls++;
         CK(cudaGetLastError());
     }
     if (!mb.empty()) {
         mel_group_kernel<<<(unsigned)mb.size(), MEL_THREADS, kMelSmemBytes, g->s_mel>>>(tables, (const MelGroupBlock*)(g->up.p + o_mb));
-        ctx->launches++; g->calls++;
+        ctx->launches++; g->steps.calls++;
         CK(cudaGetLastError());
     }
     // the detection launched so far is read back within the same wait
     if (!g->det_busy.empty()) {
         CK(cudaStreamWaitEvent(g->s_mel, g->ev_det, 0));
-        g->calls++;
+        g->steps.calls++;
     }
     // every flag in one copy: the round's host wait (the upload's pinned buffer and host pcm are read by then)
     CK(cudaMemcpyAsync(g->nan_host.p, g->nan, (size_t)g->n_slots * 4, cudaMemcpyDeviceToHost, g->s_mel));
     CK(cudaEventRecord(g->ev_mel, g->s_mel));
     CK(cudaEventSynchronize(g->ev_mel));
     CK(cudaStreamWaitEvent(st, g->ev_mel, 0));
-    g->calls += 3; g->waits++;
+    g->steps.calls += 3; g->steps.waits++;
     group_det_resolve(g);
 
     const int* flags = (const int*)g->nan_host.p;
     for (size_t i = 0; i < items.size(); ++i) {
         GroupItem& it = items[i];
-        const Plan1& p = pl[i];
-        if (p.L < 0 || (p.piece == 0 && p.L == it.s->mel.L && !p.fin)) continue;
+        const MelPiece& p = pl[i];
+        if (!live[i]) continue;
         GroupSession* s = it.s;
-        if (s->mel.resampling()) { s->mel.clk = p.clk; s->mel.n_in += p.piece; }
-        s->mel.L = p.L;
-        s->mel.f_next = std::max(s->mel.f_next, p.f_end);
-        it.done += p.piece;
+        s->mel.commit(p);
+        it.done += p.n;
         if (it.done < it.n || (it.finish && !p.fin)) *more = true;
         auto fail_session = [&](const std::string& msg) {   // its rows of this tick do not run
             s->failed = true;
@@ -590,10 +429,10 @@ static int group_round(w2l_stream_group* g, std::vector<GroupItem>& items, std::
         for (long long r = it.first + it.queued; r < a.n_fixed; ++r, ++it.queued)
             pend->push_back(GroupPend{s, &it.rows[(size_t)(r - it.first) * W2L_STREAM_ROW],
                                       it.out + (size_t)(r - it.first) * frame_bytes});
-        if (p.fin) s->finished = true;
     }
     size_t k = 0;
-    for (; pend->size() - k >= (size_t)g->max_batch; k += g->max_batch) CKR(group_step(g, pend->data() + k, g->max_batch, st));
+    const int B = g->steps.max_batch;
+    for (; pend->size() - k >= (size_t)B; k += B) CKR(group_step(g, pend->data() + k, B, st));
     pend->erase(pend->begin(), pend->begin() + k);
     return W2L_OK;
 }
@@ -617,7 +456,7 @@ static int group_tick(w2l_stream_group* g, int n, const int32_t* ids, const floa
         first_index[i] = s->emitted;
         n_out[i] = 0;
         if (s->failed) { status[i] = W2L_EINVAL; continue; }
-        if (s->finished) return fail(W2L_ESTATE, "session %d is finished", ids[i]);
+        if (s->mel.finished) return fail(W2L_ESTATE, "session %d is finished", ids[i]);
         const long long ns = n_samples[i];
         const float* p = pcm ? pcm[i] : nullptr;
         if (ns < 0 || (ns > 0 && !p)) return fail(W2L_EINVAL, "session %d: bad audio piece (%lld samples)", ids[i], ns);
@@ -655,7 +494,7 @@ static int group_tick(w2l_stream_group* g, int n, const int32_t* ids, const floa
     upto.clear();
     for (const GroupItem& it : items) {
         GroupSession* s = it.s;
-        if (!s || !s->detect || s->failed || s->finished) continue;
+        if (!s || !s->detect || s->failed || s->mel.finished) continue;
         StreamSched::At a;
         CKR(s->sched.at(s->mel.L + kDetAheadSamples, false, &a));
         upto.push_back({s, s->sched.need(a)});
@@ -686,22 +525,14 @@ int w2l_stream_group_create(w2l_ctx* ctx, int max_batch, int audio_ring_log2, w2
     DeviceGuard dg(ctx->device);
     std::unique_ptr<w2l_stream_group> g(new w2l_stream_group());
     g->ctx = ctx;
-    g->max_batch = max_batch;
     g->ring_log2 = audio_ring_log2 ? audio_ring_log2 : 16;
     CKR(g->s_mel.create());
-    CKR(g->cap.create());
     CKR(g->ev_mel.create());
     CKR(g->ev_caller.create());
     CKR(g->s_det.create());
     CKR(g->ev_det.create());
     CKR(g->ev_open.create());
-    for (Event& e : g->table_done) CKR(e.create());
-    for (Event& e : g->step_done) CKR(e.create());
-    CKR(g->table.grow(ctx, (size_t)max_batch * sizeof(GroupRow)));
-    CKR(g->table_host.alloc((size_t)kGroupSlots * max_batch * sizeof(GroupRow)));
-    CKR(g->chunks.grow(ctx, (size_t)max_batch * 1280 * 4));
-    CKR(g->crops.grow(ctx, (size_t)max_batch * 96 * 96 * 3));
-    CKR(g->preds.grow(ctx, (size_t)max_batch * 96 * 96 * 3));
+    CKR(g->steps.init(ctx, max_batch));
     CKR(group_nan_capacity(g.get(), 1));
     *out = g.release();
     return W2L_OK;
@@ -714,13 +545,7 @@ static int group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_
     DeviceGuard dg(ctx->device);
     std::unique_ptr<GroupSession> s(new GroupSession());
     CKR(s->sched.init(d, rects_host, detect));
-    if ((long long)d->H * d->W * 3 > INT32_MAX) return fail(W2L_EINVAL, "a %dx%d frame: need fewer than 2^31 bytes", d->H, d->W);
-    cudaPointerAttributes pa;
-    const cudaError_t e = cudaPointerGetAttributes(&pa, frames_dev);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(W2L_EINVAL, "frames: cudaPointerGetAttributes: %s", cudaGetErrorString(e)); }
-    if (pa.type != cudaMemoryTypeDevice || pa.device != ctx->device)
-        return fail(W2L_EINVAL, "frames must be device memory of the context's device %d", ctx->device);
-    if (!ctx->nets[W2L_NET_GENERATOR].loaded) return fail(W2L_ESTATE, "generator weights not loaded");
+    CKR(check_stream_frames(ctx, frames_dev, *d));
     if (detect) {
         if (!ctx->nets[W2L_NET_S3FD].loaded) return fail(W2L_ESTATE, "S3FD weights not loaded");
         if (d->H < 32 || d->W < 32) return fail(W2L_EINVAL, "S3FD needs frames of at least 32 x 32, got %dx%d", d->H, d->W);
@@ -730,7 +555,7 @@ static int group_open(w2l_stream_group* g, const uint8_t* frames_dev, const w2l_
     s->frames = frames_dev;
     // as the session's: the frames of every row not yet run (< max_batch + 4 chunks) beside a whole audio ring of new ones
     const long long ra = 1LL << g->ring_log2;
-    CKR(s->mel.init(ctx, g->ring_log2, (long long)std::ceil((g->max_batch + 4) * s->sched.mult) + 64 + ra / MEL_HOP + 16));
+    CKR(s->mel.init(ctx, g->ring_log2, (long long)std::ceil((g->steps.max_batch + 4) * s->sched.mult) + 64 + ra / MEL_HOP + 16));
     int slot;
     if (!g->free_slots.empty()) { slot = g->free_slots.back(); g->free_slots.pop_back(); }
     else { CKR(group_nan_capacity(g, g->n_slots + 1)); slot = g->n_slots++; }
@@ -800,7 +625,7 @@ int w2l_stream_group_pending(const w2l_stream_group* g, int n, const int32_t* id
         if (f == g->sessions.end()) return fail(W2L_EINVAL, "session %d is not open in this group", ids[i]);
         const GroupSession* s = f->second.get();
         n_out[i] = 0;
-        if (s->failed || s->finished) continue;
+        if (s->failed || s->mel.finished) continue;
         if (n_samples[i] < 0) return fail(W2L_EINVAL, "session %d: bad audio piece (%lld samples)", ids[i], (long long)n_samples[i]);
         StreamSched::At a;
         CKR(s->sched.at(s->mel.samples_after(n_samples[i], finish && finish[i] != 0), finish && finish[i] != 0, &a));
@@ -823,9 +648,9 @@ const char* w2l_stream_group_error(const w2l_stream_group* g, int32_t session_id
 
 int w2l_stream_group_counters(const w2l_stream_group* g, int64_t* calls, int64_t* host_waits, int64_t* steps) {
     if (!g) return fail(W2L_EINVAL, "null argument");
-    if (calls) *calls = g->calls;
-    if (host_waits) *host_waits = g->waits;
-    if (steps) *steps = g->steps;
+    if (calls) *calls = g->steps.calls;
+    if (host_waits) *host_waits = g->steps.waits;
+    if (steps) *steps = g->steps.count;
     return W2L_OK;
 }
 
@@ -833,7 +658,7 @@ int w2l_stream_group_destroy(w2l_stream_group* g) {
     if (!g) return W2L_OK;
     DeviceGuard dg(g->ctx->device);
     cudaDeviceSynchronize();   // queued steps may still read the group's buffers
-    for (auto& b : g->buckets) group_release(g, b.get());
+    for (auto& b : g->buckets) g->steps.release(b.get());
     for (const DetPlan& p : g->det_plans)
         if (p.plan && p.epoch == g->ctx->plan_epoch[W2L_NET_S3FD]) p.plan->pins--;
     delete g;

@@ -1,8 +1,7 @@
-// stream.cuh — the kernels of a streaming lip-sync step that the offline path does not have: the 16-frame mel
-// chunks of a step's rows gathered out of the session's mel ring (mel.cuh, mel_ring_kernel) into the (N,1,80,16) layout
-// the generator reads.  Chunk starts are absolute mel frame indices, read from the step's device table, so the launch
-// itself has no per-step arguments and can be replayed from a CUDA graph.  For stream groups (many sessions per step),
-// the audio scatter into many rings and per-row forms of the gather, the crop and the paste.
+// stream.cuh — the kernels of a streaming lip-sync step that the offline path does not have, for the lone session
+// (w2l_stream_*) and stream groups (w2l_stream_group_*) alike: the 16-frame mel chunks of a step's rows gathered out of
+// their sessions' mel rings (mel.cuh, mel_ring_kernel) into the (N,1,80,16) layout the generator reads, and per-row
+// forms of the offline crop and paste; for stream groups, the audio scatter into many rings.
 #pragma once
 
 #include <stdint.h>
@@ -11,18 +10,9 @@
 
 namespace w2l {
 
-// out[n][m][t] = ring[m][(starts[n] + t) & (pitch - 1)]
-__global__ void mel_ring_gather_kernel(const float* ring, long long pitch, const int* starts, int N, float* out) {
-    const int total = N * 80 * 16;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const int t = i & 15, m = (i >> 4) % 80, n = i / 1280;
-        out[i] = ring[(long long)m * pitch + (((long long)__ldg(starts + n) + t) & (pitch - 1))];
-    }
-}
-
-// ---- stream groups (w2l_stream_group_*): the rows of one step come from many sessions ----
 // Every pointer a step reads or writes is in its device table, one GroupRow per row, so the whole step (gather, crop,
-// generator, paste) is captured once per bucket size and replayed whatever sessions the rows belong to.
+// generator, paste) is captured once per bucket size and replayed whatever sessions the rows belong to.  Chunk starts
+// are absolute mel frame indices.
 struct GroupRow {
     const float* mel;        // the session's mel ring, (80, pitch) row-major by absolute frame
     long long pitch;
@@ -32,9 +22,10 @@ struct GroupRow {
     int H, W, frame, y1, y2, x1, x2, pad;
 };
 
-// One tick's new samples of one session (blockIdx.y) into its audio ring at absolute positions [at, at + n).
+// A piece of one session's new samples into its audio ring (or its input ring, when it resamples) at absolute
+// positions [at, at + n): copied by the lone session, one block row (blockIdx.y) of group_scatter_kernel in a group.
 struct GroupScatter {
-    const float* src;        // the packed upload (host pcm) or the caller's device pcm
+    const float* src;        // the caller's pcm; in a group, host pcm is read from the packed upload
     float* ring;
     long long mask, at, n;
 };
@@ -45,7 +36,7 @@ __global__ void group_scatter_kernel(const GroupScatter* d) {
         s.ring[(s.at + i) & s.mask] = __ldg(s.src + i);
 }
 
-// mel_ring_gather_kernel with a ring per row
+// out[n][m][t] = ring_n[m][(start_n + t) & (pitch_n - 1)]
 __global__ void group_gather_kernel(const GroupRow* rows, int N, float* out) {
     const int total = N * 80 * 16;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
