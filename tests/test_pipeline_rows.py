@@ -146,6 +146,52 @@ def test_resize_oracle_against_live_opencv():
             H = W = 96
         img = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
         assert np.array_equal(P.resize_linear_u8(img, (dw, dh)), cv2.resize(img, (dw, dh))), (H, W, dh, dw)
+    # video frames: crops of face-sized and edge boxes down to 96 x 96 (2 to 40x), and 96 x 96 pastes up to the box
+    pred = rng.integers(0, 256, (96, 96, 3), dtype=np.uint8)
+    for H, W in ((720, 1280), (1080, 1920), (2160, 3840), (1079, 1917)):
+        frame = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+        boxes = [(0, H, 0, W), (H - 1, H, 0, W), (0, H, W - 1, W)]
+        for k in range(12):
+            h, w = (int(v) for v in rng.integers(60, min(H, 900) + 1, 2))
+            y1, x1 = (0, 0) if k % 4 == 0 else (H - h, W - w) if k % 4 == 1 else (int(rng.integers(0, H - h + 1)),
+                                                                                  int(rng.integers(0, W - w + 1)))
+            boxes.append((y1, y1 + h, x1, x1 + w))
+        for y1, y2, x1, x2 in boxes:
+            crop = frame[y1:y2, x1:x2]
+            assert np.array_equal(P.resize_linear_u8(crop, (96, 96)), cv2.resize(crop, (96, 96))), (H, W, y1, y2, x1, x2)
+            if (y2 - y1) * (x2 - x1) <= 1200 * 1200:       # the whole-frame pastes are in resize_video.json
+                assert np.array_equal(P.resize_linear_u8(pred, (x2 - x1, y2 - y1)), cv2.resize(pred, (x2 - x1, y2 - y1))), \
+                    (H, W, y1, y2, x1, x2)
+
+
+def _video_gold(golden_dir):
+    import json
+    import os
+    with open(os.path.join(golden_dir, "resize_video.json")) as f:
+        return json.load(f)["cases"]
+
+
+def _video_gold_output(case, resize):
+    """resize(src, dsize) on the seeded source of one resize_video.json case (tests/golden/make_golden_resize.py)"""
+    if case["kind"] == "crop":
+        (H, W), (y1, y2, x1, x2) = case["frame"], case["box"]
+        return resize(_gold_image(H, W, case["seed"])[y1:y2, x1:x2], (96, 96))
+    h, w = case["size"]
+    return resize(_gold_image(96, 96, case["seed"]), (w, h))
+
+
+def _sha256(a):
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint8).tobytes()).hexdigest()
+
+
+def test_resize_oracle_is_pinned_to_opencv_digests_at_video_sizes(golden_dir):
+    """The oracle's crops and pastes at 720p, 1080p, 4K and 1079 x 1917 hash to the SHA-256 of cv2.resize's output
+    (tests/golden/resize_video.json, made by cv2 itself)."""
+    cases = _video_gold(golden_dir)
+    assert len(cases) >= 20
+    for case in cases:
+        assert _sha256(_video_gold_output(case, P.resize_linear_u8)) == case["sha256"], case
 
 
 @pytest.mark.gpu
