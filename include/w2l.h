@@ -563,8 +563,9 @@ int w2l_debug_train_blocks(w2l_ctx* ctx, int net, int cap, w2l_train_block_info*
 /* One tape tensor of block `block` (forward order) of the last training plan of `net`, as fp32 NCHW with exactly the
  * stored 16-bit values: X input, Z pre-BatchNorm conv output, Y output, DY its gradient, DZ gradient of Z (of the conv
  * output), DU gradient of the residual branch, DX input gradient, DX_ADD the skip gradient added to it; STATS is the
- * batch statistics (n = 2: mean, invstd; c = cout; h = w = 1) in fp32.  *n,*c,*h,*w receive the dims (any may be NULL);
- * out_dev == NULL only queries them.  A tensor the block does not have is W2L_EINVAL. */
+ * batch statistics (n = 2: mean, invstd; c = cout; h = w = 1) in fp32; F32 is the fp32 copy of Y that SyncNet's last
+ * audio and face blocks keep for the embedding normalisation (n = N, c = cout, h = w = 1).  *n,*c,*h,*w receive the dims
+ * (any may be NULL); out_dev == NULL only queries them.  A tensor the block does not have is W2L_EINVAL. */
 #define W2L_TAPE_X      0
 #define W2L_TAPE_Z      1
 #define W2L_TAPE_Y      2
@@ -574,6 +575,7 @@ int w2l_debug_train_blocks(w2l_ctx* ctx, int net, int cap, w2l_train_block_info*
 #define W2L_TAPE_DX     6
 #define W2L_TAPE_DX_ADD 7
 #define W2L_TAPE_STATS  8
+#define W2L_TAPE_F32    9
 int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* out_dev, int* n, int* c, int* h, int* w,
                            void* stream);
 

@@ -48,7 +48,7 @@ EXPORTS = [
 STREAM_ROW = 7  # W2L_STREAM_ROW: output index, chunk start, frame index, y1, y2, x1, x2
 KFAM_IGEMM, KFAM_PATCH, KFAM_CONVT_FUSED = 0, 1, 2
 WG_PLAIN, WG_STRIDED, WG_TRANSPOSED, WG_SWAP, WG_FOLDED = 0, 1, 2, 3, 4
-TAPE_X, TAPE_Z, TAPE_Y, TAPE_DY, TAPE_DZ, TAPE_DU, TAPE_DX, TAPE_DX_ADD, TAPE_STATS = range(9)
+TAPE_X, TAPE_Z, TAPE_Y, TAPE_DY, TAPE_DZ, TAPE_DU, TAPE_DX, TAPE_DX_ADD, TAPE_STATS, TAPE_F32 = range(10)
 
 
 class W2LError(RuntimeError):
@@ -312,7 +312,8 @@ class Context:
 
     def train_tensor(self, net: int, block: int, which: int, stream: int = 0):
         """One tape tensor of a block of the last training plan of `net` (TAPE_*) as a float32 CUDA tensor (NCHW; STATS:
-        (2, C, 1, 1) = mean, invstd), or None if the block has no such tensor.  Synchronises `stream`."""
+        (2, C, 1, 1) = mean, invstd; F32: the fp32 output of SyncNet's last blocks, (N, C, 1, 1)), or None if the block
+        has no such tensor.  Synchronises `stream`."""
         import torch
         d = [C.c_int32() for _ in range(4)]
         r = self.lib.w2l_debug_train_tensor(self.h, int(net), int(block), int(which), None, *[C.byref(v) for v in d], None)

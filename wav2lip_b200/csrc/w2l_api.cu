@@ -1352,7 +1352,17 @@ int w2l_debug_train_tensor(w2l_ctx* ctx, int net, int block, int which, float* o
         case W2L_TAPE_DX: a = &b.dx; C = b.L.cin; break;
         case W2L_TAPE_DX_ADD: a = &b.dx_add; C = b.L.cin; break;
         case W2L_TAPE_STATS: break;
+        case W2L_TAPE_F32: break;
         default: return fail(W2L_EINVAL, "unknown tape tensor %d", which);
+    }
+    if (which == W2L_TAPE_F32) {   // dense [N][cout] fp32 (bn_apply_kernel's y_f32)
+        if (!b.y_f32 || b.y.H != 1 || b.y.W != 1) return fail(W2L_EINVAL, "%s has no fp32 output", b.L.name.c_str());
+        if (n) *n = b.y.N;
+        if (c) *c = C;
+        if (h) *h = 1;
+        if (w) *w = 1;
+        if (out) CK(cudaMemcpyAsync(out, b.y_f32, (size_t)b.y.N * C * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+        return W2L_OK;
     }
     if (which == W2L_TAPE_STATS) {
         if (!b.bn) return fail(W2L_EINVAL, "%s has no BatchNorm statistics", b.L.name.c_str());
