@@ -423,12 +423,19 @@ typedef struct w2l_kernel_info {
     int32_t family;     /* W2L_KFAM_* */
     int32_t bn, bk, mt, head, bf16, x2, tma_epi, fold;
     int32_t m_tiles, n_tiles, grid;
+    int32_t box_w, box_h, box_n;  /* output pixels of one M tile: width x height x images (patch / fused convT: one image) */
+    int32_t patch_th;   /* patch kernel: output rows per tile; 0 for the other families */
 } w2l_kernel_info;
 /* every compiled conv kernel instantiation (generic, patch, fused transposed conv); host only */
 int w2l_debug_kernel_table(int cap, w2l_kernel_info* out);
 /* the conv launches of the last plan of `net`; net = -1: of the last w2l_conv_block_forward call */
 int w2l_debug_plan_kernels(w2l_ctx* ctx, int net, int cap, w2l_kernel_info* out);
 /* Both return the number of entries written (at most cap), or a negative W2L_E* code; out == NULL returns the count. */
+/* Build later inference plans as if the device had n SMs (persistent grids of at most n CTAs, and every dispatch choice
+ * that depends on the SM count), so that the dispatch of a smaller part can be run on a larger one.  1 <= n <= the
+ * device's own count, or 0 to restore that count; W2L_EINVAL otherwise.  Drops every cached inference plan of the context;
+ * training plans built earlier keep their grids.  Synchronises the device. */
+int w2l_debug_set_sm_count(w2l_ctx* ctx, int n);
 /* The sorted pre-NMS candidates (score > 0.5) of `image` of the last S3FD call, which must have been w2l_s3fd_detect_u8:
  * min(n, cap) rows of x1 y1 x2 y2 score location-index to HOST memory, *n = all candidates of the image, *nms_path = 0 if
  * its NMS ran in shared memory, 1 if in global memory.  Synchronises the device. */

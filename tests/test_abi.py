@@ -1,6 +1,7 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library loads and exports every symbol
 include/w2l.h declares, the architecture tables match the oracle's independent statement, the
 Python mirrors carry the reference's state_dict keys, and the product never touches oracle/."""
+import ctypes as C
 import os
 import re
 import subprocess
@@ -35,6 +36,25 @@ def test_library_exports_every_declared_symbol(lib):
         assert hasattr(L, s), f"{s} declared in include/w2l.h but not exported by libw2l.so"
     assert sorted(lib.EXPORTS) == syms, "wav2lip_b200/_lib.py EXPORTS out of sync with include/w2l.h"
     assert L.w2l_abi_version() == 1
+
+
+def test_kernel_info_binding_matches_header(lib):
+    """w2l_kernel_info is filled field by field by the library and read through ctypes (also inside
+    w2l_train_block_info): the binding must list the header's fields in the header's order, box shape and patch tile
+    height last."""
+    src = open(os.path.join(ROOT, "include", "w2l.h")).read()
+    body = re.search(r"typedef struct w2l_kernel_info \{(.*?)\} w2l_kernel_info;", src, flags=re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    fields = []
+    for decl in body.split(";"):
+        decl = decl.strip()
+        if decl:
+            fields += [re.sub(r"\[.*\]", "", f).strip() for f in re.sub(r"^\w+\s+", "", decl).split(",")]
+    assert [f for f, _ in lib.KernelInfo._fields_] == fields
+    assert fields[-4:] == ["box_w", "box_h", "box_n", "patch_th"]
+    assert C.sizeof(lib.KernelInfo) == 64 + 4 * (len(fields) - 1)
+    rows = lib.kernel_table()
+    assert rows and all(r["box_w"] == r["box_h"] == r["box_n"] == r["patch_th"] == 0 for r in rows)
 
 
 def test_library_is_sm90a_wgmma_tma(lib):

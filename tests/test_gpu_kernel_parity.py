@@ -714,17 +714,22 @@ def _export(ctx, net, i):
     return y
 
 
-def _check_chain(ctx, net, layers, sd, inputs, prec, items, what):
-    """layers: [(name, row)] in table order; inputs: name -> float32 block input (or a callable of the exports)."""
+def _check_chain(ctx, net, layers, sd, inputs, prec, items, what, trim=False):
+    """layers: [(name, row)] in table order; inputs: name -> float32 block input (or a callable of the exports).
+    trim: keep only the rows `items` of every export (large batches); `inputs` then sees the trimmed exports and must
+    return trimmed caller tensors too."""
     outs, worst = {}, 0.0
+    sel = slice(None) if trim else items
     for i, (name, row) in enumerate(layers):
         y = _export(ctx, net, i)
+        if trim and y is not None:
+            y = y[items]
         outs[name] = y
         x = inputs(name, outs)
         if y is None or x is None:
             continue
-        ref, mag = reference(x[items], sd, name, row, prec)
-        worst = max(worst, compare(y[items], ref, mag, prec, f"{what} {name}")[0])
+        ref, mag = reference(x[sel], sd, name, row, prec)
+        worst = max(worst, compare(y[sel], ref, mag, prec, f"{what} {name}")[0])
     return outs, worst
 
 
@@ -755,7 +760,7 @@ def _generator_inputs(mel, face, prec):
     return layers, inputs
 
 
-def _run_generator(prec, off, N, items):
+def _run_generator(prec, off, N, items, trim=False):
     from wav2lip_b200 import _lib
     ctx = _ctx(prec, off)
     ctx.set_debug(True)
@@ -772,11 +777,12 @@ def _run_generator(prec, off, N, items):
     if prec == F16:
         assert not ctx.f16_overflow(clear=True)
     ks = ctx.plan_kernels(_lib.NET_GENERATOR)
-    layers, inputs = _generator_inputs(mel, face, prec)
-    outs, worst = _check_chain(ctx, _lib.NET_GENERATOR, layers, sd, inputs, prec, items, f"generator {off or 'all-on'}")
+    layers, inputs = _generator_inputs(mel[items], face[items], prec) if trim else _generator_inputs(mel, face, prec)
+    outs, worst = _check_chain(ctx, _lib.NET_GENERATOR, layers, sd, inputs, prec, items, f"generator {off or 'all-on'}",
+                               trim)
     # output block + fused head: the block output stays fp32 inside the head -> sigmoid(W . relu(block) + b) in float64
     name, row = layers[-1]
-    x = inputs(name, outs)[items]
+    x = inputs(name, outs)[slice(None) if trim else items]
     blk, mag = reference(x, sd, name, row, prec, round_out=False)
     hw = sd["output_block.1.weight"].to("cuda", torch.float64).view(3, 32)
     hb = sd["output_block.1.bias"].to("cuda", torch.float64)

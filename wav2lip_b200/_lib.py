@@ -33,7 +33,7 @@ EXPORTS = [
     "w2l_train_bind", "w2l_train_forward", "w2l_train_backward", "w2l_adam_step", "w2l_wav2lip_train_step",
     "w2l_hq_wav2lip_train_step", "w2l_syncnet_train_step", "w2l_adam_state",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
-    "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
+    "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_set_sm_count", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
     "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
     "w2l_resample_num_samples", "w2l_resample", "w2l_resample_filter_host", "w2l_resample_final",
     "w2l_melstream_create", "w2l_melstream_pending", "w2l_melstream_push", "w2l_melstream_finish", "w2l_melstream_destroy",
@@ -70,7 +70,8 @@ class LayerInfo(C.Structure):
 class KernelInfo(C.Structure):
     _fields_ = [("name", C.c_char * 64), ("family", C.c_int32), ("bn", C.c_int32), ("bk", C.c_int32), ("mt", C.c_int32),
                 ("head", C.c_int32), ("bf16", C.c_int32), ("x2", C.c_int32), ("tma_epi", C.c_int32), ("fold", C.c_int32),
-                ("m_tiles", C.c_int32), ("n_tiles", C.c_int32), ("grid", C.c_int32)]
+                ("m_tiles", C.c_int32), ("n_tiles", C.c_int32), ("grid", C.c_int32),
+                ("box_w", C.c_int32), ("box_h", C.c_int32), ("box_n", C.c_int32), ("patch_th", C.c_int32)]
 
     def as_dict(self) -> dict:
         d = {f: getattr(self, f) for f, _ in self._fields_}
@@ -193,6 +194,7 @@ def get_lib() -> C.CDLL:
     lib.w2l_conv_block_train.argtypes = [vp, C.POINTER(LayerInfo), vp, i32, i32, i32] + [vp] * 14
     lib.w2l_debug_kernel_table.argtypes = [i32, C.POINTER(KernelInfo)]
     lib.w2l_debug_plan_kernels.argtypes = [vp, i32, i32, C.POINTER(KernelInfo)]
+    lib.w2l_debug_set_sm_count.argtypes = [vp, i32]
     lib.w2l_debug_train_blocks.argtypes = [vp, i32, i32, C.POINTER(TrainBlockInfo)]
     lib.w2l_debug_train_tensor.argtypes = [vp, i32, i32, i32, vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
                                            C.POINTER(i32), vp]
@@ -298,6 +300,10 @@ class Context:
     def plan_kernels(self, net: int) -> list:
         """The conv launches of the last plan of `net` (-1: of the last w2l_conv_block_forward) as a list of dicts."""
         return _kernel_rows(lambda cap, out: self.lib.w2l_debug_plan_kernels(self.h, int(net), cap, out))
+
+    def set_sm_count(self, n: int):
+        """Build later inference plans for n SMs (1 .. the device's count; 0 restores it); drops the cached plans."""
+        check(self.lib.w2l_debug_set_sm_count(self.h, int(n)))
 
     def train_blocks(self, net: int) -> list:
         """The blocks of the last training plan of `net` (-1: of the last w2l_conv_block_train) as a list of dicts."""

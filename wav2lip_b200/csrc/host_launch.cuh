@@ -100,6 +100,10 @@ static void op_kernel_info(const w2l_ctx* ctx, const Op& op, w2l_kernel_info* k)
     k->tma_epi = (!op.ctf && !op.patch && op.cp.tma_epi) ? 1 : 0;
     k->fold = op.fold ? 1 : 0;
     k->m_tiles = op.m_tiles; k->n_tiles = op.n_tiles; k->grid = op.grid;
+    // the box of output pixels one M tile covers (width x height x images)
+    if (op.ctf) { k->box_w = 8; k->box_h = 16; k->box_n = 1; }
+    else if (op.patch) { k->box_w = kPatchTileW; k->box_h = op.patch_th; k->box_n = 1; k->patch_th = op.patch_th; }
+    else { k->box_w = op.cp.bw; k->box_h = op.cp.bh; k->box_n = op.cp.bn; }
 }
 
 static int launch_conv(w2l_ctx* ctx, const Op& op, cudaStream_t st, bool pdl = true) {

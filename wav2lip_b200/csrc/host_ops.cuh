@@ -218,7 +218,7 @@ static int make_patch_op(w2l_ctx* ctx, Plan* pl, const ConvArgs& a, const PatchG
     }
     const long long total = (long long)h.tiles_x * h.tiles_y * a.in.N;
     op.grid = (int)std::min<long long>(total, ctx->num_sms);
-    op.fold = w.fold; op.m_tiles = (int)total; op.n_tiles = 1;
+    op.fold = w.fold; op.m_tiles = (int)total; op.n_tiles = 1; op.patch_th = g.TH;
     op.flops = 2.0 * a.macs_per_pixel * (double)a.Wl * a.Hl * a.in.N;
     pl->ops.push_back(op);
     return W2L_OK;

@@ -194,6 +194,7 @@ struct Op {
     ConvTParams tp;
     bool fold = false;  // K-folded first layer
     int m_tiles = 0, n_tiles = 0;  // output tiles along pixels / channels (w2l_debug_plan_kernels)
+    int patch_th = 0;    // patch kernel: output rows per tile (kPatchTileH, or kChTileH in the channel-major form)
     // ingest
     IngestParams ip;
     int ingest_src = 0;  // which caller tensor: 0 = mel / frames, 1 = face
@@ -241,7 +242,8 @@ struct w2l_ctx {
     int device = 0;
     bool bf16 = false;
     bool x2 = false;        // W2L_PREC_F32X: split fp16 operands (hi + lo), generic kernel only
-    int num_sms = 132;
+    int num_sms = 132;      // SMs plans are built for: the device's own count unless w2l_debug_set_sm_count lowered it
+    int device_sms = 132;   // the device's own count
     bool keep_all = false;  // debug: no buffer reuse, every layer output stays readable
     bool use_patch = true;   // W2L_DISABLE_HALO=1 turns the patch kernel off (A/B testing)
     bool use_mt2 = true;    // W2L_DISABLE_MT2=1

@@ -97,7 +97,7 @@ int w2l_create(int device, int precision, w2l_ctx** out) {
     ctx->device = device;
     ctx->bf16 = precision == W2L_PREC_BF16;
     ctx->x2 = precision == W2L_PREC_F32X;
-    ctx->num_sms = prop.multiProcessorCount;
+    ctx->num_sms = ctx->device_sms = prop.multiProcessorCount;
     for (Stream* s : {&ctx->stream, &ctx->s_h2d, &ctx->s_d2h, &ctx->s_side}) CKR(s->create());
     for (Event* e : {&ctx->ev_rs, &ctx->ev_fork, &ctx->ev_join, &ctx->ev_in[0], &ctx->ev_done[0], &ctx->ev_out[0], &ctx->ev_in[1],
                      &ctx->ev_done[1], &ctx->ev_out[1]})
@@ -699,6 +699,17 @@ int w2l_debug_plan_kernels(w2l_ctx* ctx, int net, int cap, w2l_kernel_info* out)
     const int k = std::min<int>(std::max(cap, 0), (int)t.size());
     for (int i = 0; i < k; ++i) out[i] = t[i];
     return k;
+}
+
+int w2l_debug_set_sm_count(w2l_ctx* ctx, int n) {
+    if (!ctx) return fail(W2L_EINVAL, "null ctx");
+    // a persistent grid of fewer CTAs than SMs is always legal; more than the device has is never built
+    if (n < 0 || n > ctx->device_sms) return fail(W2L_EINVAL, "SM count %d outside 1..%d (0: the device's own)", n, ctx->device_sms);
+    DeviceGuard g(ctx->device);
+    CK(cudaDeviceSynchronize());  // queued forwards still use the plans' buffers
+    ctx->num_sms = n == 0 ? ctx->device_sms : n;
+    for (int net = 0; net < 4; ++net) drop_plans(ctx, net);
+    return W2L_OK;
 }
 
 int w2l_debug_layer_output(w2l_ctx* ctx, int net, int layer, float* y, int* n, int* c, int* h, int* w, void* stream) {
