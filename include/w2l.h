@@ -180,6 +180,24 @@ int w2l_s3fd_forward(w2l_ctx* ctx, const float* img_dev, float* const* outs12_de
 int w2l_s3fd_detect_u8(w2l_ctx* ctx, const uint8_t* frames_dev, int B, int H, int W, int reverse_channels, int max_det,
                        float* dets_dev, int32_t* counts_dev, float* const* outs12_dev, void* stream);
 
+/* preprocess.py's per-frame work after the detector (preprocess.py:38-67, its abort handling :82-89, and the box rules of
+ * face_detection/api.py:64-79), on the device and with no host sync:
+ *   frames (B,H,W,3) uint8 on the device, frame b being frame frame0 + b of its video; dets (B,max_det,5) / counts (B) as
+ *   w2l_s3fd_detect_u8 writes them (any device buffer of that layout; only each image's first box is read).  frame0 must be a
+ *   multiple of batch (--batch_size): the video's calls cover whole detector batches, except its last one.
+ *   state int32[2] (device or pinned): next free slot, abort frame (INT32_MAX: none).  Zero it once per video; consecutive
+ *   calls of the video continue from it (a call at frame0 = 0 does not read the abort frame).
+ *   -> rows (B,6) int32 (device or pinned): status (0 kept, 1 no face, 2 non-finite box, 3 empty crop, 4 lost after the
+ *      video's abort), slot (-1 unless kept), y1, y2, x1, x2: the slice bounds after np.clip(d, 0, None), int() and NumPy's
+ *      clamp to H / W (a non-finite coordinate leaves 0).  A non-finite box ends the video at the start of its batch, an
+ *      empty slice at its own frame, the earlier point wins; the frame that raised keeps status 2 / 3.
+ *   -> crops + slot*96*96*3 = cv2.resize(frame[y1:y2, x1:x2], (96, 96)) for every kept frame, bit-exact, in device or
+ *      pinned host memory.  Slots are dealt in frame order.  A slot >= cap is not written: state[0] > cap after the
+ *      video's calls reports that overflow. */
+int w2l_face_crops_u8(w2l_ctx* ctx, const uint8_t* frames_dev, int B, int H, int W, const float* dets_dev,
+                      const int32_t* counts_dev, int max_det, int frame0, int batch, int32_t* state, int32_t* rows,
+                      uint8_t* crops, int64_t cap, void* stream);
+
 /* Replaces `SyncNet_color.forward(audio, face)` (syncnet.py:55-66):
  *   mel (B,1,80,16), face (B,15,48,96) -> audio_emb (B,512), face_emb (B,512), both L2-normalised. */
 int w2l_syncnet_forward(w2l_ctx* ctx, const float* mel_dev, const float* face_dev,

@@ -61,6 +61,13 @@ with torch.no_grad():
     from wav2lip_b200.face_detection.detection.sfd.net_s3fd import s3fd
     det = s3fd().cuda().eval()
     dm = det(torch.rand(1, 3, 96, 128).cuda() * 255)
+    # preprocess.py on the device: detection, then w2l_face_crops_u8 (host frames with a padded last launch, device frames)
+    from wav2lip_b200.data import face_crops
+    from wav2lip_b200.face_detection import FaceAlignment, LandmarksType
+    fa = FaceAlignment(LandmarksType._2D, flip_input=False, device="cuda")
+    fa.face_detector.face_detector = det
+    fc_rows, fc_crops = face_crops(fa, np.random.randint(0, 256, (5, 96, 128, 3), dtype=np.uint8), batch_size=2)
+    fc_rows2, fc_crops2 = face_crops(fa, torch.randint(0, 256, (3, 96, 128, 3), dtype=torch.uint8).cuda(), batch_size=1)
     torch.cuda.synchronize()
 # scope row f1: one training iteration through the autograd bridge and one fused native step (B=1, T=5)
 from wav2lip_b200.training import Wav2LipTrainStep

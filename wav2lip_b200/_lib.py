@@ -34,7 +34,7 @@ EXPORTS = [
     "w2l_hq_wav2lip_train_step", "w2l_syncnet_train_step", "w2l_adam_state",
     "w2l_train_last_output", "w2l_train_flops", "w2l_comm_unique_id", "w2l_comm_init", "w2l_conv_block_train", "w2l_train_profile",
     "w2l_debug_kernel_table", "w2l_debug_plan_kernels", "w2l_debug_set_sm_count", "w2l_debug_train_blocks", "w2l_debug_train_tensor",
-    "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
+    "w2l_s3fd_detect_u8", "w2l_debug_s3fd_candidates", "w2l_face_crops_u8", "w2l_train_batch_wav2lip", "w2l_train_batch_syncnet",
     "w2l_resample_num_samples", "w2l_resample", "w2l_resample_filter_host", "w2l_resample_final",
     "w2l_melstream_create", "w2l_melstream_pending", "w2l_melstream_push", "w2l_melstream_finish", "w2l_melstream_destroy",
     "w2l_melstream_set_input_rate", "w2l_stream_set_input_rate", "w2l_stream_group_set_input_rate",
@@ -172,6 +172,7 @@ def get_lib() -> C.CDLL:
     lib.w2l_s3fd_forward.argtypes = [vp, vp, C.POINTER(vp), i32, i32, i32, vp]
     lib.w2l_s3fd_detect_u8.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, C.POINTER(vp), vp]
     lib.w2l_debug_s3fd_candidates.argtypes = [vp, i32, i32, vp, C.POINTER(i32), C.POINTER(i32)]
+    lib.w2l_face_crops_u8.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, i64, vp]
     lib.w2l_crop_resize_u8.argtypes = [vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_paste_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]
     lib.w2l_lipsync_frames_u8.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(i32), i32, vp, vp]

@@ -28,6 +28,7 @@
 #include "resample.cuh"
 #include "netspec.h"
 #include "resize.cuh"
+#include "face_crops.cuh"
 #include "s3fd_detect.cuh"
 #include "stream.cuh"
 #include "train_data.cuh"
@@ -503,6 +504,32 @@ int w2l_s3fd_detect_u8(w2l_ctx* ctx, const uint8_t* frames, int B, int H, int W,
     CKR(ensure_s3fd_detect(ctx, pl));
     const S3fdRun run{frames, reverse_channels, max_det, dets, counts};
     return run_plan(ctx, pl, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream, false, outs, &run);
+}
+
+// preprocess.py's per-frame step after the detector: rows, slots and 96x96 crops, no host sync (face_crops.cuh)
+int w2l_face_crops_u8(w2l_ctx* ctx, const uint8_t* frames, int B, int H, int W, const float* dets, const int32_t* counts,
+                      int max_det, int frame0, int batch, int32_t* state, int32_t* rows, uint8_t* crops, int64_t cap,
+                      void* stream) {
+    if (!ctx || !frames || !dets || !counts || !state || !rows || !crops) return fail(W2L_EINVAL, "null argument");
+    if (B <= 0 || H <= 0 || W <= 0) return fail(W2L_EINVAL, "bad shape B=%d H=%d W=%d", B, H, W);
+    if (max_det < 1) return fail(W2L_EINVAL, "max_det must be at least 1, got %d", max_det);
+    if (batch < 1) return fail(W2L_EINVAL, "batch must be at least 1, got %d", batch);
+    if (frame0 < 0 || frame0 % batch != 0) return fail(W2L_EINVAL, "frame0 %d is not a non-negative multiple of batch %d", frame0, batch);
+    if ((int64_t)frame0 + B >= kFcNoAbort) return fail(W2L_EINVAL, "frame0 %d + B %d does not fit int32", frame0, B);
+    if (cap < 0) return fail(W2L_EINVAL, "negative cap %lld", (long long)cap);
+    const void* cd = nullptr;
+    CKR(train_source(ctx, crops, "crops", &cd));
+    DeviceGuard g(ctx->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const FaceCropParams p{frames, dets, counts, state, rows, (uint8_t*)cd, (long long)cap, B, H, W, max_det, frame0, batch};
+    face_crops_rows_kernel<<<1, kFcThreads, 0, st>>>(p);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    const dim3 grid((kFcPix + kFcResizeThreads - 1) / kFcResizeThreads, std::min(B, 65535));
+    face_crops_resize_kernel<<<grid, kFcResizeThreads, 0, st>>>(p);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return W2L_OK;
 }
 
 int w2l_debug_s3fd_candidates(w2l_ctx* ctx, int image, int cap, float* out, int* n, int* nms_path) {

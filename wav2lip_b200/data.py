@@ -20,6 +20,18 @@ re-reads ten jpgs, re-resizes them and recomputes the whole utterance's mel for 
   reference's draw order depends on torch's per-worker seeds; that order is not reproduced, only the sampling distribution.
 
 Host decode (`scan_data_root`, `decode_video`) is separate from the device part.  There is no CPU fallback for the latter.
+
+preprocess.py itself (the step that makes the jpgs) also runs on the device, from decoded videos:
+
+  cache = TrainDataCache.from_videos(({"path": p, "frames": f, "wav": w, "sr": sr} for ...), FaceAlignment(...))
+
+* `face_crops` is preprocess.py's `process_video_file` (:38-67, with mp_handler's abort rules :82-89) for one video: the S3FD
+  detector (`w2l_s3fd_detect_u8`) and `w2l_face_crops_u8` leave a row per frame (kept / no face / non-finite box / empty crop /
+  lost after the video's abort, and the slice bounds) and `cv2.resize(frame[y1:y2, x1:x2], (96, 96))` of every kept frame on
+  the device, with no host sync until the rows are read.  `from_videos` builds the cache from them, names `{i}.jpg` as the
+  script's files.  Deliberate deviation: the cache holds the resize of the raw crop, where the reference's training data went
+  through a JPEG round trip (`cv2.imwrite`, then `cv2.imread` in the Dataset).  `write_face_crops` writes the script's files
+  byte for byte from the same rows instead, for the reference's own scripts or `from_data_root`.
 """
 from __future__ import annotations
 
@@ -39,6 +51,7 @@ IMG = 96                 # hparams.img_size
 SAMPLE_RATE = 16000      # hparams.sample_rate
 W2L_FIELDS, SYNC_FIELDS = 17, 8   # sample-row widths of include/w2l.h w2l_train_batch_wav2lip / _syncnet
 _CANVAS_BYTES = 64 << 20          # host canvas per resize launch
+_LAUNCH_PIXELS = 1 << 22          # frame pixels per detector launch of face_crops (DESIGN.md section 3.12)
 
 
 def get_image_list(data_root: str, split: str, filelist: str = None) -> list:
@@ -77,6 +90,106 @@ def decode_video(vid: str, img_names: list, pool: ThreadPoolExecutor = None) -> 
     except Exception:
         wav = None
     return {"path": vid, "img_names": img_names, "crops": crops, "wav": wav}
+
+
+def _cache_device(storage, device):
+    import torch
+    if storage not in ("device", "pinned"):
+        raise ValueError(f"storage must be 'device' or 'pinned', got {storage!r}")
+    return torch.device("cuda", torch.cuda.current_device() if device is None else torch.device(device).index or 0)
+
+
+def _launch_frames(H: int, W: int, batch_size: int) -> int:
+    """Frames per detector launch in `face_crops`: batch_size * 2^k, the most that stay within _LAUNCH_PIXELS frame pixels
+    (at least batch_size), so that every launch starts at a multiple of batch_size and a frame size has one S3FD plan."""
+    n = batch_size
+    while 2 * n * H * W <= _LAUNCH_PIXELS:
+        n *= 2
+    return n
+
+
+def face_crops(detector, frames, batch_size: int = 32, out=None):
+    """preprocess.py's `process_video_file` (:38-67) for one video on the device, up to the jpgs: frames (F,H,W,3) uint8 BGR
+    (host memory or a CUDA tensor), `detector` this package's `face_detection.FaceAlignment`, `batch_size` the script's
+    --batch_size, which only sets where a non-finite box ends the video (mp_handler, :82-89).
+    -> rows (F, 6) int32 ndarray, one per frame: status (0 kept, 1 no face, 2 non-finite box, 3 empty crop, 4 lost after the
+       video's abort), slot (-1 unless kept), y1, y2, x1, x2 (include/w2l.h w2l_face_crops_u8; oracle/preprocess_oracle.py);
+       crops (n_kept, 96, 96, 3) uint8 = cv2.resize(frame[y1:y2, x1:x2], (96, 96)) of the kept frames in frame order, in
+       `out` (uint8 (cap, 96, 96, 3), device or pinned host memory; default: a new device tensor of F slots).
+    The detector sees each frame as get_detections_for_batch does (channels reversed), in launches sized from H x W (the top
+    box of an image does not depend on its batch, DESIGN.md section 3.6), the last one padded.  Host frames are staged
+    through pinned memory.  The host waits only once, for the rows, at the end."""
+    import torch
+    from . import _lib
+    if isinstance(batch_size, bool) or int(batch_size) != batch_size or batch_size < 1:
+        raise ValueError(f"batch_size must be a positive int, got {batch_size!r}")
+    batch_size = int(batch_size)
+    net = detector.face_detector.face_detector           # FaceAlignment -> SFDDetector -> the s3fd module
+    dev = next(net.parameters()).device
+    if dev.type != "cuda":
+        raise ValueError("the detector must be on a CUDA device")
+    x = frames if isinstance(frames, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(np.asarray(frames)))
+    if x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != 3:
+        raise ValueError(f"expected (F,H,W,3) uint8 frames, got {x.dtype} {tuple(x.shape)}")
+    if x.is_cuda and x.device != dev:
+        raise ValueError(f"frames are on {x.device}, the detector on {dev}")
+    x = x.contiguous()
+    F, H, W, _ = x.shape
+    if out is None:
+        out = torch.empty((F, IMG, IMG, 3), dtype=torch.uint8, device=dev)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or tuple(out.shape[1:]) != (IMG, IMG, 3) \
+            or not out.is_contiguous() or not (out.device == dev or (not out.is_cuda and out.is_pinned())):
+        raise ValueError(f"out must be a contiguous uint8 (cap, 96, 96, 3) tensor on {dev} or in pinned host memory")
+    rows = torch.empty((F, 6), dtype=torch.int32, device=dev)
+    if F == 0:
+        return rows.cpu().numpy(), out[:0]
+    L = _launch_frames(H, W, batch_size)
+    state = torch.zeros((2,), dtype=torch.int32, device=dev)
+    pad = None
+    stream = torch.cuda.current_stream(dev)
+
+    def p(t):
+        return C.c_void_p(t.data_ptr())
+    with torch.no_grad(), torch.cuda.device(dev):
+        for s in range(0, F, L):
+            n = min(L, F - s)
+            if x.is_cuda and n == L:
+                src = x[s:s + L]
+            else:
+                if pad is None:
+                    pad = torch.zeros((L, H, W, 3), dtype=torch.uint8, device=dev)
+                if x.is_cuda:
+                    pad[:n].copy_(x[s:s + n])
+                else:   # a fresh block of the caching host allocator, reused once its copy has completed
+                    stage = torch.empty((n, H, W, 3), dtype=torch.uint8, pin_memory=True)
+                    stage.copy_(x[s:s + n])
+                    pad[:n].copy_(stage, non_blocking=True)
+                src = pad
+            dets, counts, _ = net.detect_u8(src, 1, reverse_channels=True)
+            ctx = net._w2l_ctx
+            _lib.check(ctx.lib.w2l_face_crops_u8(ctx.h, p(src), n, H, W, p(dets), p(counts), 1, s, batch_size, p(state),
+                                                 p(rows[s:]), p(out), out.shape[0], C.c_void_p(stream.cuda_stream)))
+    st = state.cpu().numpy()
+    rows = rows.cpu().numpy()
+    if int(st[0]) > out.shape[0]:
+        raise ValueError(f"{int(st[0])} kept frames do not fit the {out.shape[0]} slots of out")
+    return rows, out[:int(st[0])]
+
+
+def write_face_crops(fulldir: str, frames, rows) -> list:
+    """preprocess.py's files from `face_crops`' rows, on the host: cv2.imwrite(join(fulldir, "{i}.jpg"), frame[y1:y2, x1:x2])
+    for every kept frame i (preprocess.py:67), byte-identical to the script's for the same boxes.  -> the names written."""
+    import cv2
+    os.makedirs(fulldir, exist_ok=True)
+    if hasattr(frames, "cpu"):
+        frames = frames.cpu().numpy()
+    names = []
+    for i, r in enumerate(np.asarray(rows)):
+        if r[0] == 0:
+            names.append("{}.jpg".format(i))
+            if not cv2.imwrite(join(fulldir, names[-1]), frames[i][r[2]:r[3], r[4]:r[5]]):
+                raise OSError(f"cv2.imwrite failed for {join(fulldir, names[-1])}")
+    return names
 
 
 class VideoIndex:
@@ -191,18 +304,62 @@ class TrainDataCache:
         return cls._build([(v.get("path", str(i)), v["img_names"]) for i, v in enumerate(videos)], videos, storage, device)
 
     @classmethod
-    def _build(cls, scan, decoded, storage, device):
+    def from_videos(cls, videos, detector, batch_size: int = 32, storage: str = "device", device=None) -> "TrainDataCache":
+        """preprocess.py and then the cache, on the device: videos yields one dict per video with "frames" ((F,H,W,3) uint8
+        BGR, host memory or a CUDA tensor), "wav" (float samples, None = the audio failed), "sr" (default 16000) and "path".
+        `detector` is this package's `face_detection.FaceAlignment`, `batch_size` preprocess.py's --batch_size.  Each video's
+        kept frames are `face_crops`' crops, named "{i}.jpg" by frame index; its mel is melspectrogram(resample(wav, sr,
+        16000)), as the Dataset's load_wav of the script's audio.wav gives it.  The frames are the 96x96 resize of the raw
+        crop, without the reference's JPEG round trip (DESIGN.md section 3.12)."""
+        import torch
+        from . import audio
+        dev = _cache_device(storage, device)
+
+        def alloc(n):
+            return torch.empty((n, IMG, IMG, 3), dtype=torch.uint8, device=dev) if storage == "device" else \
+                torch.empty((n, IMG, IMG, 3), dtype=torch.uint8, pin_memory=True)
+        buf, used, scan, decoded = alloc(0), 0, [], []
+        for i, v in enumerate(videos):
+            frames = v["frames"]
+            F = len(frames)
+            if used + F > buf.shape[0]:           # grow geometrically: the kernel writes straight into the cache
+                nb = alloc(max(used + F, 2 * buf.shape[0]))
+                nb[:used].copy_(buf[:used])
+                buf = nb
+            rows, _ = face_crops(detector, frames, batch_size, out=buf[used:used + F])
+            names = ["{}.jpg".format(j) for j in np.flatnonzero(rows[:, 0] == 0)]
+            wav, sr = v.get("wav"), int(v.get("sr", SAMPLE_RATE))
+            if wav is not None and sr != SAMPLE_RATE:
+                try:
+                    w = wav if isinstance(wav, torch.Tensor) else torch.as_tensor(np.asarray(wav, dtype=np.float32))
+                    wav = audio.resample(w.to(dev, torch.float32), sr, SAMPLE_RATE)
+                except Exception:     # load_wav raises on such audio: the video keeps its frames and loses its audio
+                    wav = None
+            path = v.get("path", str(i))
+            scan.append((path, names))
+            decoded.append({"path": path, "img_names": names, "slots": range(used, used + len(names)), "wav": wav})
+            used += len(names)
+        if used != buf.shape[0]:
+            buf = alloc(used).copy_(buf[:used])
+        return cls._build(scan, decoded, storage, dev, frames=buf)
+
+    @classmethod
+    def _build(cls, scan, decoded, storage, device, frames=None):
+        """frames: None (resize every decoded crop into a new cache), or the finished cache, whose slots each decoded
+        video gives as "slots"."""
         import torch
         from . import _lib, audio
-        if storage not in ("device", "pinned"):
-            raise ValueError(f"storage must be 'device' or 'pinned', got {storage!r}")
-        dev = torch.device("cuda", torch.cuda.current_device() if device is None else torch.device(device).index or 0)
+        dev = _cache_device(storage, device)
         n = sum(len(names) for _, names in scan)
         if n == 0:
             raise ValueError("the dataset has no *.jpg frames")
         shape = (n, IMG, IMG, 3)
-        frames = torch.zeros(shape, dtype=torch.uint8, device=dev) if storage == "device" else \
-            torch.zeros(shape, dtype=torch.uint8).pin_memory()
+        given = frames is not None
+        if not given:
+            frames = torch.zeros(shape, dtype=torch.uint8, device=dev) if storage == "device" else \
+                torch.zeros(shape, dtype=torch.uint8).pin_memory()
+        elif tuple(frames.shape) != shape:
+            raise ValueError(f"expected a frame cache of shape {shape}, got {tuple(frames.shape)}")
         ctx = audio._context(dev.index)
         stream = torch.cuda.current_stream(dev)
         pending, canvas_hw = [], [0, 0]   # (slot, crop) waiting for the next resize launch, and their canvas's (h, w)
@@ -231,8 +388,8 @@ class TrainDataCache:
 
         index, mels, slot, mel_off = [], [], 0, 0
         for (path, names), v in zip(scan, decoded):
-            slots = []
-            for c in v["crops"]:
+            slots = [int(k) for k in v["slots"]] if given else []
+            for c in ([] if given else v["crops"]):
                 if c is None:
                     slots.append(-1)
                 else:
@@ -278,7 +435,9 @@ class TrainDataCache:
         if wav is None:
             return None
         try:
-            return audio.melspectrogram(torch.as_tensor(np.asarray(wav, dtype=np.float32)).to(dev)).t().contiguous()
+            w = wav.to(dev, torch.float32) if isinstance(wav, torch.Tensor) and wav.is_cuda else \
+                torch.as_tensor(np.asarray(wav, dtype=np.float32)).to(dev)
+            return audio.melspectrogram(w).t().contiguous()
         except Exception:
             return None
 
